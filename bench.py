@@ -2,7 +2,7 @@
 """bench.py -- contigs/sec of the vamb hot path (VAE train + encode + medoid clustering).
 
 Contract (one JSON line on rank 0):
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--scaling strong|weak]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--scaling strong|weak] [--dump-outputs DIR]
 
 Workload: BASELINE.json configs[1] -- 1,000,000 planted contigs x (103 TNF + 50 abundance samples), `vamb bin
 default` settings (VAE 512-512-32, 300 epochs, batch 256 doubling at epochs 25/75/150/225, then
@@ -26,6 +26,11 @@ N > 1 (torchrun, one rank per GPU):
   --scaling weak: every rank owns its own 1M-contig sample (own genomes); same data-parallel training, encode and
       clustering per shard (Vamb splits bins per sample).
 
+--dump-outputs DIR: after the timed pass, what its last step computed, as DIR/<name>.npy (float32 / float64, < 64 MB):
+the latent of a fixed seeded sample of rows (all rows up to LATENT_SAMPLE), those row indices, the cluster ordinal of
+every contig (clusters numbered in the order the generator yields them) and the medoid of every cluster.  Rank 0
+writes them: with --scaling strong it clusters the gathered latent of all contigs, with --scaling weak its own sample.
+
 --impl reference: the CPU port of the reference path (oracle/) on the host cores, ONE bounded sample of the same
 workload (a few optimiser steps per batch size, encode of 50k rows, the first clusters), extrapolated over the
 schedule and labelled as such.  It never imports the product package.
@@ -48,12 +53,13 @@ import torch  # noqa: E402
 
 METRIC = "contigs/sec (VAE train + cluster) at N=1M, S=50"
 BATCHSTEPS = [25, 75, 150, 225]
+LATENT_SAMPLE = 262_144  # latent rows written by --dump-outputs (32 MB at 32 dimensions)
 
 
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps (>= 1): slices of the one timed pass")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"])
@@ -67,7 +73,12 @@ def parse_args():
     ap.add_argument("--time-budget", type=float, default=780.0,
                     help="wall-clock budget (s): optional legs (e2e, cpu_baseline) are skipped, and say so, when the run "
                          "would exceed it")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the latent (seeded row sample) and the clusters of the timed pass as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 def schedule(n: int, nepochs: int, batch0: int = 256):
@@ -83,7 +94,7 @@ def schedule(n: int, nepochs: int, batch0: int = 256):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -142,53 +153,22 @@ def make_workload(n, nsamples, seed):
 
 
 def workload_name(args) -> str:
-    """The same string on both arms (the driver compares the `config` of the two JSON lines)."""
+    """The same string on both arms, so that the `config` of the two JSON lines can be compared."""
     return (f"{args.n} contigs x (103 TNF + {args.nsamples} abundance), bin default VAE 512-512-32, {args.nepochs} "
             "epochs (batch 256 doubling at 25/75/150/225) + encode + medoid clustering to exhaustion")
 
 
 def reference_threads() -> int:
     """The reference caps its BLAS/OpenMP threads at min(ncpu, 8) (vamb/__main__.py:27-40, 2221-2228); more threads
-    oversubscribe these small kernels (the 128-thread run on the GPU box was far slower per step)."""
+    oversubscribe these small kernels."""
     return min(os.cpu_count() or 8, 8)
 
 
-def measured_peaks():
-    """(HBM GB/s, tensor TFLOP/s, tensor peak label).  HBM: MEASURED_PEAKS.json (driver-written copy bandwidth).
-    Tensor: the TF32 dense cuBLAS peak measured on this pool's B200 by tools/measure_tf32_peak.py
-    (profiles/r02_tf32_peak.json, tracked) -- these GEMMs are kind::tf32; else half the measured BF16 figure."""
-    hbm, bf16, which = 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
-            p = json.load(fh)
-        hbm, bf16, which = float(p["hbm_gbs"]), float(p["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:
-        pass
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_tf32_peak.json")) as fh:
-            t = json.load(fh)
-        return hbm, float(t["tf32_tflops_sustained"]), "measured cuBLAS TF32 8192^3 sustained (profiles/r02_tf32_peak.json)", which
-    except Exception:
-        return hbm, bf16 / 2.0, f"half of the {which} bf16 dense sustained figure (no TF32 measurement on file)", which
-
-
-def ncu_record(kernel: str):
-    """The committed ncu capture of `kernel` (tools/ncu_extract.py -> profiles/r02_ncu_traffic.json): dram bytes per
-    launch, tensor-pipe activity, duration under the profiler -- or None when no capture is on file."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")) as fh:
-            t = json.load(fh)
-        for k, v in t.items():
-            if kernel.startswith(k) or k.startswith(kernel):
-                return v if isinstance(v, dict) else {"dram_bytes": v}
-    except Exception:
-        pass
-    return None
-
-
-def ncu_traffic(kernel: str):
-    r = ncu_record(kernel)
-    return None if r is None else r.get("dram_bytes")
+def datasheet_peaks():
+    """(HBM GB/s, tensor TFLOP/s, tensor peak label, HBM peak label): NVIDIA's H100 SXM data sheet (700 W card), dense
+    TF32 -- these GEMMs are wgmma .tf32.  A card with a lower power limit (see "clocks") reaches less."""
+    return (3350.0, 495.0, "H100 SXM data sheet, dense TF32 (not reached: an upper bound)",
+            "H100 SXM data sheet HBM3 (not reached: an upper bound)")
 
 
 # ---------------------------------------------------------------------------------- the GPU pass
@@ -242,6 +222,7 @@ def run_pass(ctx: Ctx, dl, lengths_cluster, nepochs, k_steps, resident: bool, ma
     ctx.barrier()
     step_ms, phases = [], {"train": 0.0, "encode": 0.0, "cluster": 0.0}
     n_clusters = n_members = probes = evals = 0
+    medoids, members = [], []  # kept for --dump-outputs only
     cluster_timing = {}
     latent_dev = None
     t_wall0 = time.perf_counter()
@@ -284,6 +265,9 @@ def run_pass(ctx: Ctx, dl, lengths_cluster, nepochs, k_steps, resident: bool, ma
                 for c in gen:
                     n_clusters += 1
                     n_members += len(c.members)
+                    if args.dump_outputs and ctx.rank == 0:
+                        medoids.append(int(c.medoid))
+                        members.append(np.asarray(c.members))
                     if max_clusters and n_clusters >= max_clusters:
                         break
                 probes, evals = gen._n_probes, gen._n_evals
@@ -312,7 +296,23 @@ def run_pass(ctx: Ctx, dl, lengths_cluster, nepochs, k_steps, resident: bool, ma
             "n_clusters": n_clusters, "n_clustered": n_members, "probes": probes, "evals": evals,
             "train_steps": sum(s * e for _, s, e in sched), "launches": launches,
             "final_loss": vae._last_epoch_losses[0], "vae": vae, "latent_dev": latent_dev,
-            "cluster_timing": cluster_timing}
+            "cluster_timing": cluster_timing, "medoids": medoids, "members": members}
+
+
+def dump_outputs(outdir: str, res, n_rows: int, seed: int) -> None:
+    """What the timed pass computed in its last step (see --dump-outputs), as .npy files under `outdir`."""
+    os.makedirs(outdir, exist_ok=True)
+    rows = np.arange(n_rows)
+    if n_rows > LATENT_SAMPLE:
+        rows = np.sort(np.random.default_rng(seed).choice(n_rows, LATENT_SAMPLE, replace=False))
+    latent = res["latent_dev"][torch.from_numpy(rows).cuda()].cpu().numpy().astype(np.float32)
+    cluster_of = np.full(n_rows, -1.0, dtype=np.float64)
+    for k, m in enumerate(res["members"]):
+        cluster_of[m] = k
+    np.save(os.path.join(outdir, "latent_sample.npy"), latent)
+    np.save(os.path.join(outdir, "latent_sample_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(outdir, "cluster_of_contig.npy"), cluster_of)
+    np.save(os.path.join(outdir, "cluster_medoid.npy"), np.asarray(res["medoids"], dtype=np.float64))
 
 
 def vae_roofline(vae, n, nepochs):
@@ -365,7 +365,7 @@ def probe_roofline(latent_dev, lengths):
         call(i)
     times = []
     for i in range(10):
-        flush.zero_()  # > L2 (126 MB): the next probe reads from HBM
+        flush.zero_()  # > L2 (50 MB): the next probe reads from HBM
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         call(i + 3)
@@ -521,8 +521,11 @@ def main():
     sampler = ClockSampler(ctx.local_rank)
     sampler.start()
     log(f"timed pass: {args.steps} steps (dataset resident in HBM)")
-    res = run_pass(ctx, dl, lens_cluster, args.nepochs, max(1, args.steps), resident=True)
+    res = run_pass(ctx, dl, lens_cluster, args.nepochs, args.steps, resident=True)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0 and res["latent_dev"] is not None:  # weak scaling: rank 0's own sample
+        dump_outputs(args.dump_outputs, res, len(lens_cluster), args.seed)
+        log(f"outputs of the timed pass written to {args.dump_outputs}")
     t_pass = ctx.max_over_ranks(res["t_event"])
     value = n_total / t_pass
     log(f"  {t_pass:.2f}s: train {res['phases']['train']:.2f} encode {res['phases']['encode']:.2f} cluster "
@@ -550,22 +553,21 @@ def main():
                "api": "make_dataloader tensors (pinned host) -> VAE.trainmodel -> VAE.encode -> numpy -> ClusterGenerator"}
 
     if rank == 0:
-        hbm_peak, tf_peak, tf_label, hbm_label = measured_peaks()
+        hbm_peak, tf_peak, tf_label, hbm_label = datasheet_peaks()
         log("kernel rooflines")
         best, share = vae_roofline(res["vae"], len(dl.dataset.tensors[0]), args.nepochs)
         roof = {"bound": "tensor", "kernel": best["kernel"], "achieved": best["tflops"], "peak": tf_peak,
-                "unit": "TFLOP/s", "frac": best["tflops"] / tf_peak, "traffic": ncu_traffic(best["kernel"].split("[")[0]),
+                "unit": "TFLOP/s", "frac": best["tflops"] / tf_peak, "traffic": None,
                 "peak_source": tf_label, "time_share": share, "ms_per_launch": best["ms"],
-                "ncu": ncu_record(best["kernel"].split("[")[0]),  # committed capture: tensor-pipe % / dram bytes of this kernel
                 "note": "algorithmic FLOP of the launch (wgrad + dgrad, SURVEY 8d) / CUDA-event time of the launch; the tensor "
                         "pipe executes 3x these FLOP (3xTF32 error compensation)"}
         roof_cluster = None
         if res["latent_dev"] is not None:
             pr = probe_roofline(res["latent_dev"], lens_cluster)
             roof_cluster = {"bound": "hbm", "kernel": pr["kernel"], "achieved": pr["gbs"], "peak": hbm_peak,
-                            "unit": "GB/s", "frac": pr["gbs"] / hbm_peak, "traffic": ncu_traffic("probe_kernel"),
+                            "unit": "GB/s", "frac": pr["gbs"] / hbm_peak, "traffic": None,
                             "algorithmic_bytes": pr["bytes"], "ms_per_launch": pr["ms"],
-                            "peak_source": f"{hbm_label} copy bandwidth"}
+                            "peak_source": hbm_label}
             log(f"  dominant {best['kernel']}: {best['tflops']:.1f} TFLOP/s; probe {pr['gbs']:.0f} GB/s")
         base = None
         if world == 1:

@@ -1,4 +1,4 @@
-/* vamb_b200 -- C ABI of the B200 (sm_100a) kernels behind the vamb hot path.
+/* vamb_b200 -- C ABI of the H100 (sm_90a) kernels behind the vamb hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference (RasmussenLab/vamb) is
  * pure Python + PyTorch and has no FFI of its own; the functions below are what a
@@ -35,7 +35,7 @@ extern "C" {
 
 const char *vk_last_error(void);
 int vk_abi_version(void);
-/* sm_100a-only build: returns 0 when the current device can run these kernels. */
+/* sm_90a-only build: returns 0 when the current device can run these kernels. */
 int vk_check_device(void);
 
 /* ------------------------------------------------------------------ clustering */
@@ -292,7 +292,7 @@ typedef struct vk_vae {
     vk_vae_ctl *ctl;
     vk_vae_layer layers[VK_VAE_MAX_LAYERS];
     int32_t data_ld;                    /* floats per dataset row (>= d_in; a multiple of 4 keeps rows 16-byte aligned) */
-    int32_t tc_min_batch;               /* batches >= this run the GEMMs on tcgen05 (3xTF32); 0 = never            */
+    int32_t tc_min_batch;               /* batches >= this run the GEMMs on wgmma (3xTF32); 0 = never              */
     int64_t grad_slab;                  /* floats between the split-K gradient slabs of `grads`                    */
     int32_t n_grad_slabs;               /* slabs allocated in `grads` (>= 1)                                       */
     int32_t staging;                    /* tensor-core operand staging: 0 = fused into the producing kernels' epilogues
@@ -348,7 +348,7 @@ int vk_vae_profile_step(const vk_vae *net, int batch, const vk_vae_inject *injec
 /* Backward + gradients only (no optimiser): used by the multi-GPU path and by the tests. */
 int vk_vae_grad_step(const vk_vae *net, int batch, const vk_vae_inject *inject, void *stream);
 
-/* Stand-alone check of the PRODUCTION tcgen05 3xTF32 main loop (tc::ws_mainloop -- the loop of the layer kernels):
+/* Stand-alone check of the PRODUCTION wgmma 3xTF32 main loop (tc::ws_mainloop -- the loop of the layer kernels):
  * C[M,N] = A * B^T over k-tiles [kt0, kt0 + nk) of 32.  A_lane: the 128-row operand in the lane-major staging layout
  * (vk_lane_major_index), zero padded to whole 128-row panels; B: plain row-major [rows][ldb], zero padded to whole
  * tile_n-row tiles; lda, ldb multiples of 32; tile_n (output columns per CTA) a multiple of 16 in [16, 128].

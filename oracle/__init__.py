@@ -8,8 +8,8 @@ CUDA extension is missing.
 
 Contents
 --------
-ref_loader.py      load the UNMODIFIED reference files from /root/reference
-                   (present in the build container only) under a stub ``vamb``
+ref_loader.py      load the UNMODIFIED reference files from a checkout named by
+                   VAMB_REFERENCE_ROOT (golden generators only) under a stub ``vamb``
                    package with two shims (vambcore, dadaptation).
 dadapt.py          restatement of dadaptation==3.2 DAdaptAdam (parity unpinned:
                    upstream source is not available offline).

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE -- build recipe for the oracle's C inner loops.
 
-gcc only; output goes to oracle/_build/ (git-ignored, travels to the GPU box).
+gcc only; output goes to oracle/_build/ (git-ignored, built by build()).
 ``-ffp-contract=off`` keeps every a*b+c unfused unless written as fmaf();
 ``-mfma`` makes fmaf() a single hardware instruction (IEEE-exact either way).
 """

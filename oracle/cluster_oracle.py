@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE -- CPU oracle for the medoid clusterer.
 
-A restatement of /root/reference/vamb/cluster.py (CPU path, ``cuda=False``) in
+A restatement of vamb/cluster.py (CPU path, ``cuda=False``) in
 NumPy + C (oracle/csrc/oracle_kernels.c).  It follows the reference's *sequential*
 algorithm literally -- one full distance scan per ``sample_medoid`` call, physical
 row packing after every emitted cluster -- so that it is an independent check of

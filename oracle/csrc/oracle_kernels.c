@@ -2,10 +2,10 @@
  *
  * These restate, with an explicitly DEFINED floating-point order ("vk arithmetic
  * v1", DESIGN.md section 3), the tensor expressions of the reference clusterer:
- *   ok_normalize_rows  <- /root/reference/vamb/cluster.py:653-669  (_normalize)
- *   ok_dists           <- /root/reference/vamb/cluster.py:672-676  (_calc_distances)
- *   ok_sample          <- /root/reference/vamb/cluster.py:619-629  (sample_medoid body)
- *   ok_hist            <- /root/reference/vamb/cluster.py:457-481  (find_threshold head)
+ *   ok_normalize_rows  <- vamb/cluster.py:653-669  (_normalize)
+ *   ok_dists           <- vamb/cluster.py:672-676  (_calc_distances)
+ *   ok_sample          <- vamb/cluster.py:619-629  (sample_medoid body)
+ *   ok_hist            <- vamb/cluster.py:457-481  (find_threshold head)
  * The reference evaluates them with MKL sgemv / ATen reductions whose summation
  * order is undocumented; the CUDA kernels in vamb_b200/csrc implement exactly the
  * order written here, so GPU-vs-oracle parity is bit-exact by construction and

@@ -1,16 +1,16 @@
 """TEST INFRASTRUCTURE -- restatement of ``dadaptation.DAdaptAdam`` (dadaptation==3.2).
 
-The reference pins ``dadaptation==3.2`` (/root/reference/pyproject.toml:12) and
+The reference pins ``dadaptation==3.2`` (pyproject.toml:12) and
 calls ``dadaptation.DAdaptAdam(self.parameters(), decouple=True)``
-(/root/reference/vamb/encode.py:578).  The upstream source is neither in
-/root/reference nor installed here, and there is no network: this file restates
+(vamb/encode.py:578).  The upstream source is neither in
+the reference tree nor a dependency of this project: this file restates
 the published algorithm (Defazio & Mishchenko, "Learning-Rate-Free Learning by
 D-Adaptation", ICML 2023, Algorithm "Adam with D-Adaptation"; upstream file
 ``dadaptation/dadapt_adam.py`` of facebookresearch/dadaptation v3.x).
 
 PARITY UNPINNED: no golden vector of the upstream optimiser exists offline.  The
 reference tests that exercise this boundary only check that the loss falls
-(/root/reference/test/test_encode.py:152-168).  Every parity report that involves
+(test/test_encode.py:152-168).  Every parity report that involves
 the optimiser therefore says "vs the restated DAdaptAdam".
 
 Hyper-parameters as the reference uses them: lr=1.0, betas=(0.9, 0.999),

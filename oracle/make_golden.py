@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE -- generate tests/golden/*.npz from the UNMODIFIED reference.
 
-Run in the build container (needs /root/reference):  python -m oracle.make_golden
-The fixtures are small and committed; tests compare the oracle (and, on the GPU box,
+Needs a checkout of the reference:  VAMB_REFERENCE_ROOT=<checkout> python -m oracle.make_golden
+The fixtures are small and committed; tests compare the oracle (and, in the GPU tests,
 the CUDA path) against them.  Inputs are regenerated from oracle.synth with the
 seeds stored in the fixture, so only outputs are stored.
 

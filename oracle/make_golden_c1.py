@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE -- C1 trajectory fixture from the UNMODIFIED reference (BASELINE.json configs[0]).
 
-    python -m oracle.make_golden_c1 SEED      (build container only: needs /root/reference)
+    VAMB_REFERENCE_ROOT=<checkout of the reference> python -m oracle.make_golden_c1 SEED
     python -m oracle.make_golden_c1 merge     (combine the per-seed files into tests/golden/c1_trajectory.npz)
 
 Runs the live reference -- ``vamb.encode.make_dataloader`` -> ``VAE(nsamples=4, seed=SEED).trainmodel(nepochs=300,
@@ -31,7 +31,7 @@ LINE = re.compile(r"Epoch:\s*(\d+)\s+Loss:\s*(\S+)\s+CE:\s*(\S+)\s+AB:\s*(\S+)\s
 
 
 def adjusted_rand(labels_a: np.ndarray, labels_b: np.ndarray) -> float:
-    """Hubert & Arabie ARI from the contingency table (no sklearn needed on the GPU box)."""
+    """Hubert & Arabie ARI from the contingency table (no sklearn needed on the GPU machine)."""
     _, ia = np.unique(labels_a, return_inverse=True)
     _, ib = np.unique(labels_b, return_inverse=True)
     table = np.zeros((ia.max() + 1, ib.max() + 1), dtype=np.int64)

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE -- strict-RNG trajectory fixture from the UNMODIFIED reference.
 
-    python -m oracle.make_golden_strict          (build container only: needs /root/reference)
+    VAMB_REFERENCE_ROOT=<checkout of the reference> python -m oracle.make_golden_strict
 
 The live reference trains ``VAE(nsamples=4, seed=0)`` (default 512-512-32 network, dropout 0.2) on the planted
 10,000 x 4 dataset ``oracle.synth.make_contigs(10000, 4, seed=0)`` for 6 epochs with batch 256 doubling at epochs 2

@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE -- NumPy restatement of the input normalisation of the reference.
 
-Follows /root/reference/vamb/encode.py:93-126 (``make_dataloader`` up to the four tensors; the
+Follows vamb/encode.py:93-126 (``make_dataloader`` up to the four tensors; the
 DataLoader wrapping of :129-144 is not needed by the oracle, which indexes the tensors directly) and
-/root/reference/vamb/vambtools.py:250-288 (``zscore``).  Used by ``bench.py --impl reference`` and the
+vamb/vambtools.py:250-288 (``zscore``).  Used by ``bench.py --impl reference`` and the
 ``cpu_baseline`` leg so that the reference arm never imports the product package.
 tests/test_oracle_normalize.py pins it against the live reference and against the product's own
 ``vamb_b200.encode.make_dataloader`` (bit-identical tensors).

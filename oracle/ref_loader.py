@@ -1,13 +1,13 @@
 """TEST INFRASTRUCTURE -- import the UNMODIFIED reference hot-path files.
 
-Loads /root/reference/vamb/{vambtools,encode,cluster}.py by file path under a
+Loads vamb/{vambtools,encode,cluster}.py of a checkout of RasmussenLab/vamb
+(named by the environment variable VAMB_REFERENCE_ROOT) by file path under a
 stub ``vamb`` package (the real ``vamb/__init__.py`` needs an installed dist and
-wheels that are absent here), after injecting two shims into ``sys.modules``:
+compiled wheels), after injecting two shims into ``sys.modules``:
 ``vambcore`` (oracle/vambcore_shim.py) and ``dadaptation`` (oracle/dadapt.py).
 
-/root/reference exists only in the build container, never on the GPU box:
-``available()`` is False there and callers must fall back to the committed
-golden fixtures in tests/golden/.
+Only the oracle/make_golden*.py scripts use it: the tests compare with what
+those scripts recorded under tests/golden/.
 """
 from __future__ import annotations
 
@@ -16,13 +16,13 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("VAMB_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("VAMB_REFERENCE_ROOT", "")
 _PKG = "vamb"
 _cached = None
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, "vamb", "cluster.py"))
+    return bool(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, "vamb", "cluster.py"))
 
 
 def load():
@@ -31,7 +31,7 @@ def load():
     if _cached is not None:
         return _cached
     if not available():
-        raise FileNotFoundError(f"reference tree not found at {REFERENCE_ROOT}")
+        raise FileNotFoundError(f"set VAMB_REFERENCE_ROOT to a checkout of RasmussenLab/vamb (now {REFERENCE_ROOT!r})")
 
     from . import dadapt, vambcore_shim
 

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE -- torch-CPU fp32 oracle for the VAE path.
 
-A restatement of /root/reference/vamb/encode.py (``VAE`` forward, ``calc_loss``,
+A restatement of vamb/encode.py (``VAE`` forward, ``calc_loss``,
 one optimiser step, ``encode``) as a small functional model over a plain
 ``state_dict`` whose keys/shapes equal the reference's (encode.py:226-249), so
 that reference weights can be loaded and compared directly.

@@ -1,9 +1,9 @@
 """TEST INFRASTRUCTURE -- stand-in for the ``vambcore`` Rust wheel (vambcore==0.1.2,
-/root/reference/pyproject.toml:6), which is not installed here.
+pyproject.toml:6), which is not installed here.
 
-Only ``overwrite_matrix`` is on the hot path (/root/reference/vamb/vambtools.py:302,319
-<- /root/reference/vamb/cluster.py:322-328).  Its semantics are pinned by
-/root/reference/test/test_vambtools.py:271-298: rows where ``mask`` is true are
+Only ``overwrite_matrix`` is on the hot path (vamb/vambtools.py:302,319
+<- vamb/cluster.py:322-328).  Its semantics are pinned by
+test/test_vambtools.py:271-298: rows where ``mask`` is true are
 moved to the front of ``matrix`` in their original order and the number of kept
 rows is returned.  ``kmercounts`` is off-path and only stubbed.
 """

@@ -68,20 +68,18 @@ class TestDataLoader:
 
 
 def test_matches_reference_dataloader_when_available():
-    from oracle import ref_loader
+    """The reference's ``make_dataloader`` tensors on this fixture, as recorded by oracle/make_golden_live.py."""
+    import os
 
-    if not ref_loader.available():
-        pytest.skip("reference tree not present")
-    ref = ref_loader.load()
-    rng = np.random.RandomState(3)
-    tnfs = rng.random((300, 103)).astype(np.float32)
-    rpkm = rng.random((300, 5)).astype(np.float32)
-    rpkm[7] = 0
-    lens = rng.randint(2000, 90000, 300)
-    a = ref.encode.make_dataloader(rpkm.copy(), tnfs.copy(), lens, batchsize=64)
+    from oracle import make_golden_live as live
+
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_live.npz"))
+    rpkm, tnfs, lens = live.dl_fixture()
     b = ve.make_dataloader(rpkm.copy(), tnfs.copy(), lens, batchsize=64)
-    for x, y in zip(a.dataset.tensors, b.dataset.tensors):
-        assert torch.equal(x, y)
+    rows = live.norm_sample_rows(len(lens))
+    for name, y in zip("dtaw", b.dataset.tensors):
+        assert np.array_equal(y.numpy()[rows], g[f"dl_{name}_rows"]), name
+        assert live.digest(y.numpy()) == str(g[f"dl_{name}_sha256"]), name
 
 
 class TestVAEArgs:

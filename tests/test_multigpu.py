@@ -1,4 +1,4 @@
-"""2-GPU NCCL test of the row-sharded data-parallel VAE (skipped on single-GPU boxes): replicas stay
+"""2-GPU NCCL test of the row-sharded data-parallel VAE (skipped on single-GPU machines): replicas stay
 bit-identical (same gradients after the all-reduce, same optimiser state), the loss falls, and the
 per-shard encode + clustering run independently."""
 import os

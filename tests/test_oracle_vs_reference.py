@@ -1,17 +1,22 @@
 """CPU suite: the torch-fp32 VAE oracle is PINNED -- it reproduces the reference-made golden fixtures bit for bit
-(tests/golden/vae_*.npz, written by oracle/make_golden_vae.py from the unmodified reference), and, where the
-reference tree is present (build container), the live reference itself.  Also pins oracle/normalize.py."""
+(tests/golden/vae_*.npz, written by oracle/make_golden_vae.py from the unmodified reference, and
+tests/golden/reference_live.npz, written by oracle/make_golden_live.py).  Also pins oracle/normalize.py."""
+import hashlib
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import ref_loader
+from oracle import make_golden_live as live
 from oracle import vae_oracle as vo
 from oracle.make_golden_vae import VAE_CASES, vae_inputs
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+def live_golden():
+    return np.load(os.path.join(GOLDEN, "reference_live.npz"))
 
 
 def unpack_keep(packed, batch, n):
@@ -63,82 +68,68 @@ def test_normalize_restatement_matches_the_product_dataloader():
         assert np.array_equal(x, y.numpy())
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="reference tree only exists in the build container")
 def test_normalize_restatement_matches_the_live_reference():
+    """The reference's ``make_dataloader`` tensors, recorded as a SHA-256 per tensor and a sample of rows."""
     from oracle import normalize as onorm
     from oracle import synth
 
-    ref = ref_loader.load()
+    g = live_golden()
     ab, tnf, lens = synth.make_contigs(2000, 3, seed=5)
-    want = ref.encode.make_dataloader(ab.copy(), tnf.copy(), lens).dataset.tensors
-    for x, y in zip(onorm.normalize(ab, tnf, lens), want):
-        assert np.array_equal(x, y.numpy())
+    rows = live.norm_sample_rows(len(lens))
+    for name, x in zip("dtaw", onorm.normalize(ab, tnf, lens)):
+        assert np.array_equal(x[rows], g[f"norm_{name}_rows"]), name
+        assert hashlib.sha256(np.ascontiguousarray(x).tobytes()).hexdigest() == str(g[f"norm_{name}_sha256"]), name
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="reference tree only exists in the build container")
 def test_vae_oracle_equals_live_reference_over_training_steps():
     """Under the same ``torch.manual_seed`` stream the oracle and the unmodified reference stay bit-identical
-    (losses, every parameter and buffer, encode) over 6 optimiser steps."""
-    from oracle import dadapt
+    (losses, every parameter and buffer, encode) over 6 optimiser steps (the reference's run recorded by
+    oracle/make_golden_live.py)."""
+    from oracle import normalize as onorm
 
-    ref = ref_loader.load()
-    S, n, batch, seed = 5, 400, 64, 11
+    g = live_golden()
+    p = live.TRAIN
+    S, n, batch, seed = p["S"], p["n"], p["batch"], p["seed"]
     rpkm, tnfs, lens = vae_inputs(S, n, seed)
-    dl = ref.encode.make_dataloader(rpkm.copy(), tnfs.copy(), lens, batchsize=batch)
-    d, t, a, w = dl.dataset.tensors
-    vae = ref.encode.VAE(S, nhiddens=[64, 48], nlatent=12, seed=seed)
-    o = vo.OracleVAE(S, nhiddens=[64, 48], nlatent=12, seed=seed)
-    opt = dadapt.DAdaptAdam(vae.parameters(), decouple=True)
-    vae.train()
-    rng = np.random.default_rng(seed)
-    for step in range(6):
-        idx = torch.from_numpy(rng.choice(n, size=batch, replace=False).astype(np.int64))
-        torch.manual_seed(2000 + step)
-        opt.zero_grad()
-        do, to, ao, mu = vae(d[idx], t[idx], a[idx])
-        L = vae.calc_loss(d[idx], do, t[idx], to, a[idx], ao, mu, w[idx])
-        L[0].backward()
-        opt.step()
-        torch.manual_seed(2000 + step)
-        lo, _, _ = o.train_step(d[idx], t[idx], a[idx], w[idx])
-        assert [float(x.detach()) for x in L] == lo
-    for k, v in vae.state_dict().items():
-        assert torch.equal(v, o.state[k]), k
-    vae.eval()
-    assert np.array_equal(vae.encode(dl), o.encode(d, t, a, batch=batch)[0])
+    d, t, a, w = (torch.from_numpy(x) for x in onorm.normalize(rpkm, tnfs, lens))
+    threads = torch.get_num_threads()
+    torch.set_num_threads(live.THREADS)  # torch's CPU reductions split the work by thread count
+    try:
+        o = vo.OracleVAE(S, nhiddens=p["nhiddens"], nlatent=p["nlatent"], seed=seed)
+        rng = np.random.default_rng(seed)
+        for step in range(p["steps"]):
+            idx = torch.from_numpy(rng.choice(n, size=batch, replace=False).astype(np.int64))
+            torch.manual_seed(2000 + step)
+            lo, _, _ = o.train_step(d[idx], t[idx], a[idx], w[idx])
+            assert lo == list(g["train_losses"][step]), step
+        latent = o.encode(d, t, a, batch=batch)[0]
+    finally:
+        torch.set_num_threads(threads)
+    keys = [str(k) for k in g["train_state_keys"]]
+    assert keys == list(o.state)
+    for i, k in enumerate(keys):
+        assert live.digest(o.state[k].numpy()) == str(g[f"train_state_{i}_sha256"]), k
+    assert np.array_equal(latent[:16], g["train_latent_head"])
+    assert live.digest(latent) == str(g["train_latent_sha256"])
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="reference tree only exists in the build container")
 def test_strict_rng_emulation_follows_the_live_reference_trainmodel():
     """``vamb_b200.encode.reference_epoch_noise`` (the strict-RNG parity mode of the CUDA path) consumes torch's global
     generator exactly like the reference's DataLoader + forward pass: driving the (bit-exact) oracle with it reproduces
     the per-epoch losses that the unmodified ``VAE.trainmodel`` logs, including a batch-size doubling."""
-    import re
-
     pytest.importorskip("vamb_b200._lib")
-    from loguru import logger
-
     import vamb_b200.encode as ve
     from oracle import normalize as onorm
     from oracle import synth
 
-    ref = ref_loader.load()
-    S, n, seed, nepochs, bsteps = 4, 1500, 3, 4, [2]
-    ab, tnf, lens = synth.make_contigs(n, S, seed=8)
-    rows = []
-    pat = re.compile(r"Epoch:\s*(\d+)\s+Loss:\s*(\S+)")
-    logger.enable("vamb")
-    sink = logger.add(lambda m: rows.append(pat.search(str(m))), level="INFO")
-    dl = ref.encode.make_dataloader(ab.copy(), tnf.copy(), lens, batchsize=128)
-    vae = ref.encode.VAE(S, nhiddens=[64, 32], nlatent=8, seed=seed)
-    vae.trainmodel(dl, nepochs=nepochs, batchsteps=bsteps)
-    logger.remove(sink)
-    logger.disable("vamb")
-    want = [float(m.group(2)) for m in rows if m]
+    p = live.STRICT
+    S, n, seed, nepochs, bsteps = p["S"], p["n"], p["seed"], p["nepochs"], p["bsteps"]
+    ab, tnf, lens = synth.make_contigs(n, S, seed=p["data_seed"])
+    want = [float(x) for x in live_golden()["strict_epoch_losses"]]
     assert len(want) == nepochs
 
     d, t, a, w = (torch.from_numpy(x) for x in onorm.normalize(ab, tnf, lens))
-    o = vo.OracleVAE(S, nhiddens=[64, 32], nlatent=8, seed=seed)  # torch.manual_seed(seed) + the reference's init draws
+    o = vo.OracleVAE(S, nhiddens=p["nhiddens"], nlatent=p["nlatent"], seed=seed)  # torch.manual_seed(seed) + the reference's init draws
     batch, got = 128, []
     for epoch in range(nepochs):
         if epoch in bsteps:

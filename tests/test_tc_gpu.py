@@ -1,9 +1,8 @@
-"""GPU suite: the PRODUCTION tcgen05 3xTF32 main loop (tc::ws_mainloop in vk_tc.cuh -- the loop inside
-fwd_layer_tc_kernel / bwd_layer_tc_kernel: A operand in tensor memory from the lane-major staging layout, B operand
+"""GPU suite: the PRODUCTION wgmma 3xTF32 main loop (tc::ws_mainloop in vk_tc.cuh -- the loop inside
+fwd_layer_tc_kernel / bwd_layer_tc_kernel: A operand in registers from the lane-major staging layout, B operand
 through the shared-memory ring) against an fp64 reference, for every tile width, ragged shapes and split-K offsets.
-Near-fp32 accuracy is the contract: the relative error of the result matrix stays below 1e-6 + 1.2e-8 * K (measured
-4e-7 at K = 8, 4e-6 at K = 512: the tensor core's fp32 accumulator truncates, so the error grows linearly with the
-chain length; plain TF32 would sit at ~5e-4 for every K)."""
+Near-fp32 accuracy is the contract: the relative error of the result matrix stays below 1e-6 + 1.2e-8 * K (plain TF32
+would sit at ~5e-4 for every K)."""
 import numpy as np
 import pytest
 import torch
@@ -93,9 +92,8 @@ def test_lane_major_helper_matches_the_c_abi():
 @pytest.mark.parametrize("M,N,K,tile_n", [(512, 513, 512, 32), (154, 512, 4096, 64), (300, 100, 1000, 128), (128, 64, 96, 16),
                                           (128, 48, 160, 48), (256, 128, 8192, 128)])
 def test_ws_mainloop_flush_variant_matches_fp64(M, N, K, tile_n):
-    """The wgrad variant: two alternating tensor-memory accumulators, every 4 k-tiles summed into fp32 registers.  The
-    error no longer grows with the chain length: below 1e-6 + 1.2e-8 * 128 for every K, and not above the plain loop beyond
-    the short chains where the plain loop's stacked-B form (A_hi x B_lo in an accumulator of its own) is the more exact."""
+    """The wgrad variant: the tensor-core accumulation chain cut every 4 k-tiles and summed into fp32 registers.  The
+    error no longer grows with the chain length: below 1e-6 + 1.2e-8 * 128 for every K, and not above the plain loop."""
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     A = torch.randn(M, K, device="cuda", generator=g)
     B = torch.randn(N, K, device="cuda", generator=g)

@@ -98,15 +98,15 @@ def test_strict_rng_mode_follows_the_reference_trajectory():
     got = np.array(got)
     want = g["traj"]
     rel = np.abs(got - want) / np.abs(want)
-    # measured on B200: loss 2.5e-4, CE 1.2e-4, AB 4.4e-3, SSE 1.7e-3, KLD 5.9e-3 (the small parts amplify rounding)
+    # the small parts (AB, SSE, KLD) amplify rounding: a looser bound for them than for the loss
     assert rel[:, 0].max() < 5e-4, (got[:, 0], want[:, 0])
     assert rel.max() < 1.5e-2, rel.max(0)
     latent = vae.encode(dl)[:512]
-    # individual latent coordinates after 234 noisy optimiser steps: rounding differences are amplified by training (single
-    # entries differ by up to ~8 % of the largest coordinate on B200, the matrix by 9 % in Frobenius norm) although the
-    # per-epoch losses agree to 2.5e-4: the same trajectory in the large, not coordinate by coordinate
+    # individual latent coordinates after 234 noisy optimiser steps: rounding differences are amplified by training
+    # (single entries differ by several % of the largest coordinate) although the per-epoch losses agree closely: the
+    # same trajectory in the large, not coordinate by coordinate
     err = np.abs(latent - g["latent_head"]).max()
     fro = float(np.linalg.norm(latent - g["latent_head"]) / np.linalg.norm(g["latent_head"]))
     print("strict-RNG: loss rel", rel.max(0), "latent max err", err, "of", np.abs(g["latent_head"]).max(), "rel fro", fro)
-    assert fro < 0.2, fro  # measured 0.088
+    assert fro < 0.2, fro
     assert abs(float(vae.state_dict()["mu.weight"].norm()) - float(g["mu_weight_norm"])) < 1e-3 * float(g["mu_weight_norm"])

@@ -1,4 +1,4 @@
-"""Per-tensor gradient error of the tcgen05 path vs the torch-fp32 oracle (and the fp32 CUDA-core path)."""
+"""Per-tensor gradient error of the tensor-core (3xTF32) path vs the torch-fp32 oracle (and the fp32 CUDA-core path)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

@@ -1,7 +1,7 @@
 """Host cost per cluster of writing the two TSV files (SURVEY 8f-1), CPU only: the reference's per-cluster / per-member
 Python (vamb/__main__.py:1310-1377, restated in tests/test_cluster_writer_cpu.py) against the block-wise writer
 `vamb_b200.cluster.write_clusters_tsv`, on clusters shaped like the C2 job's (1M contigs in ~27k clusters).
-    python tools/writer_speed.py > profiles/r02_writer_speed.txt"""
+    python tools/writer_speed.py"""
 import os, sys, tempfile, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

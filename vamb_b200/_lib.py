@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI declared in include/vamb_b200.h.
 
 There is NO CPU fallback: importing this module without a loadable ``_vk.so`` raises, and
-``require_device()`` raises unless ``cuda:0`` is an sm_100 GPU.
+``require_device()`` raises unless ``cuda:0`` is an sm_90 (H100) GPU.
 """
 from __future__ import annotations
 
@@ -10,7 +10,7 @@ import os
 from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_uint8, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# VAMB_B200_SO selects another build of the same library (tools/kernel_timeline.py uses the stamped one)
+# VAMB_B200_SO selects another build of the same library (tools/step_timeline.py uses the stamped one)
 _SO = os.environ.get("VAMB_B200_SO") or os.path.join(_HERE, "_vk.so")
 
 VK_ABI_VERSION = 2
@@ -115,7 +115,7 @@ _device_ok = False
 
 
 def require_device() -> None:
-    """Fail loudly unless a B200-class GPU and the CUDA extension are usable."""
+    """Fail loudly unless an H100 (sm_90) GPU and the CUDA extension are usable."""
     global _device_ok
     if _device_ok:
         return
@@ -123,7 +123,7 @@ def require_device() -> None:
 
     if not torch.cuda.is_available():
         raise VkError(
-            "vamb_b200 has no CPU path: a CUDA device (sm_100, B200) is required "
+            "vamb_b200 has no CPU path: a CUDA device (sm_90, H100) is required "
             "(torch.cuda.is_available() is False)"
         )
     check(lib.vk_check_device())

@@ -1,11 +1,11 @@
-__doc__ = """Iterative medoid clustering on B200 -- drop-in for ``vamb.cluster``.
+__doc__ = """Iterative medoid clustering on H100 -- drop-in for ``vamb.cluster``.
 
 Same public surface as the reference module (RasmussenLab/vamb, vamb/cluster.py):
 ``ClusterGenerator(matrix, lengths, maxsteps, windowsize, minsuccesses, destroy,
 normalized, cuda, rng_seed)`` is an iterator of ``Cluster`` objects.  The host code
 below keeps the reference's *decision logic* (seed order, Python ``random`` call
 sequence, success window, peak/valley scan in Python floats); every O(N) tensor
-expression is a hand-written sm_100a kernel reached through the C ABI of
+expression is a hand-written sm_90a kernel reached through the C ABI of
 include/vamb_b200.h:
 
     reference (vamb/cluster.py)                this module
@@ -20,7 +20,7 @@ include/vamb_b200.h:
 Results follow the reference's CPU semantics (``cuda=False`` path, where emitted rows
 no longer exist) under "vk arithmetic v1" (DESIGN.md section 3) and are bit-identical to
 oracle/cluster_oracle.py.  There is no CPU fallback: without the CUDA extension and an
-sm_100 device construction raises.
+sm_90 device construction raises.
 """
 
 import os as _os

@@ -1,4 +1,4 @@
-// vamb_b200 clustering kernels (sm_100a).  HBM-streaming integer/compare work: no tensor
+// vamb_b200 clustering kernels (sm_90a).  HBM-streaming integer/compare work: no tensor
 // cores; the rules that matter are coalescing (8 lanes x float4 = one 128 B row, one warp =
 // 4 consecutive rows = 512 contiguous bytes per load instruction), several independent
 // loads in flight per thread, shared-memory staging of the sparse outputs, and a persistent
@@ -43,8 +43,8 @@ int vk_num_sms() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
     }
     return sms;
 }
@@ -54,8 +54,8 @@ extern "C" int vk_check_device(void) {
     VK_CUDA(cudaGetDevice(&dev));
     VK_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
     VK_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-    if (major != 10) {
-        vk_set_error("vamb_b200 kernels are built for sm_100a only; device is sm_%d%d", major, minor);
+    if (major != 9 || minor != 0) {
+        vk_set_error("vamb_b200 kernels are built for sm_90a only; device is sm_%d%d", major, minor);
         return 1;
     }
     return 0;
@@ -116,7 +116,7 @@ extern "C" int vk_check_normalized(const float *matrix, int64_t n, int d, float 
 // "Last block done" with ONE fencing thread per block: after the block barrier, thread 0's device-scope fence is
 // cumulative over everything the block wrote before the barrier (the release pattern of the PTX memory model, as in
 // cutlass/semaphore.h); having all 256 threads of every block execute MEMBAR (let alone the system-scope one, which
-// also invalidates L1) cost 30-50 us per launch on B200 (profiles/r02_ncu_summary.md: ERRBAR / barrier stalls).
+// also invalidates L1) turns every launch into a long stall on the memory barrier.
 // Returns true in every thread of the block that finishes last; that block has acquired the other blocks' writes.
 __device__ __forceinline__ bool vk_last_block(int32_t *ticket, int *s_last) {
     __syncthreads();
@@ -173,8 +173,7 @@ struct ProbeAcc {
 constexpr int PB_WBUF = 64;  // staged entries per warp (<= 16 appended per iteration)
 
 // R = independent rows (float4 loads) in flight per lane and per buffer (the chunk being processed and the next one);
-// BPS = resident blocks per SM the register budget is held to.  (A per-lane cp.async queue of 4-12 chunks in shared
-// memory was measured and dropped: 63-92 us against 45 us at N = 1M, profiles/r02_probe_sweep_v2.txt.)
+// BPS = resident blocks per SM the register budget is held to.
 template <int DFIX, int R, int BPS>
 __global__ void __launch_bounds__(PB_THREADS, BPS)
 probe_kernel(const float *__restrict__ matrix, const float *__restrict__ lengths,
@@ -247,11 +246,9 @@ probe_kernel(const float *__restrict__ matrix, const float *__restrict__ lengths
     float4 vnext[PB_R];
     // Work distribution, PER WARP and without any block barrier: a warp-chunk is 4 x R consecutive rows (one 512-byte
     // load per k for the warp, 2 KB at R = 4), a unit is `unit_chunks` warp-chunks.  Default: units strided over the
-    // warps of the grid, four chunks (8 KB) per unit (VK_PROBE_UNIT; 1 / 4 / 16 chunks: 49.9 / 49.4 / 49.5 us at N = 1M,
-    // 146 / 133 / 142 us at N = 5M) -- at any moment the grid streams one contiguous window of the matrix.  Measured alternatives (tools/probe_speed.py,
-    // profiles/r02_probe_sweep_v3.txt): units drawn from one atomic counter, two ahead (VK_PROBE_DYNAMIC=1), so that
-    // faster SMs scan more rows: 75 us against 45 us at N = 1M (the warps scheduled first claim all the units and the
-    // others idle) and 147 against 126 us at N = 5M; a block-level scheme with a barrier per unit: 54 / 164 us.
+    // warps of the grid, four chunks (8 KB) per unit (VK_PROBE_UNIT) -- at any moment the grid streams one contiguous
+    // window of the matrix.  The alternative VK_PROBE_DYNAMIC=1 draws units from one atomic counter, two ahead, so that
+    // faster SMs scan more rows (tools/probe_speed.py compares the two).
     constexpr int WCHUNK = 4 * PB_R;
     const int PB_WUNIT = unit_chunks;
     const int n_wchunks = (n32 + WCHUNK - 1) / WCHUNK;
@@ -391,7 +388,9 @@ probe_kernel(const float *__restrict__ matrix, const float *__restrict__ lengths
 }
 
 // Launch shape of the probe: rows in flight per lane (VK_PROBE_R = 4 | 8) and persistent blocks per SM
-// (VK_PROBE_BPS = 2..8); defaults chosen on B200 with tools/probe_speed.py (profiles/r02_probe_sweep.txt).
+// (VK_PROBE_BPS = 2..8).  Chosen on an H100 SXM (400 W power limit) with tools/probe_speed.py, one launch, warm L2,
+// N = 1M / 5M: R = 4 with BPS = 4 -> 71 / 242 us, BPS = 3 -> 72 / 241 us, BPS = 2 -> 76 / 263 us, BPS = 6 -> 80 / 278 us,
+// BPS = 8 -> 91 / 286 us; R = 8 with BPS = 2 -> 80 / 255 us, BPS = 4 -> 84 / 279 us.
 static int probe_env(const char *name, int dflt, int lo, int hi) {
     const char *v = getenv(name);
     const int x = v ? atoi(v) : dflt;

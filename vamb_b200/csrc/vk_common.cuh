@@ -1,4 +1,4 @@
-// Shared helpers for the vamb_b200 kernels (sm_100a only).
+// Shared helpers for the vamb_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -108,7 +108,7 @@ __device__ __forceinline__ void density_add(u64 &lo, u64 &hi, u64 len, u64 cq) {
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 // every kernel of the VAE step starts with this pair (before any global-memory access)
-// ---- optional in-kernel timeline (build with -DVK_TIMELINE; tools/kernel_timeline.py) ----
+// ---- optional in-kernel timeline (build with -DVK_TIMELINE; tools/step_timeline.py, tools/probe_timeline.py) ----
 #ifdef VK_TIMELINE
 static __device__ unsigned long long vk_tl[4096];  // per translation unit; vk_vae.cu reads its own
 static __device__ int vk_tl_base;

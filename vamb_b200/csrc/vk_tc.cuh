@@ -1,12 +1,12 @@
-// tcgen05 (5th-gen tensor core) building blocks for sm_100a: raw PTX wrappers, UMMA shared-memory /
-// instruction descriptors, and a 128 x BN x K tile GEMM in error-compensated 3xTF32.
+// Hopper (sm_90a) tensor-core building blocks: raw PTX wrappers for mbarrier, TMA and wgmma, shared-memory matrix
+// descriptors, and a 128 x BN x K tile GEMM in error-compensated 3xTF32.
 //
 // Operands are materialised ONCE per layer by the producing kernel (vk_vae.cu: fused staging / prep kernels) as
-// plain zero-padded fp32 arrays; the warp-specialised main loop below (ws_mainloop) keeps the 128-row operand in
-// tensor memory and streams the narrow operand through a shared-memory ring.
+// plain zero-padded fp32 arrays; the main loop below (ws_mainloop) feeds the 128-row operand to wgmma from registers
+// and streams the narrow operand through a shared-memory ring.
 //
-// 3xTF32: kind::tf32 reads the top 19 bits of each fp32 operand word (low 13 mantissa bits ignored),
-// so hi = x as stored, lo = x - (x & 0xFFFFE000) (exact).  D += A_hi*B_hi + A_lo*B_hi + A_hi*B_lo leaves
+// 3xTF32: a .tf32 MMA reads the top 19 bits of each fp32 operand word (low 13 mantissa bits ignored),
+// so hi = x as stored, lo = x - (x & 0xFFFFE000) (exact).  D += A_lo*B_hi + A_hi*B_lo + A_hi*B_hi leaves
 // a relative error of ~2^-21 per product, i.e. fp32-grade results from the tensor pipe.
 #pragma once
 #include "vk_common.cuh"
@@ -23,8 +23,8 @@ __device__ __forceinline__ void mbar_fence_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 // The bare try_wait loop (the hardware suspends the thread inside try_wait for a bounded time), plus a poll counter: a
-// wait that never completes (a lost arrival, a bulk copy that never lands) traps after 2^26 failed polls (seconds)
-// instead of hanging the GPU.
+// wait that never completes (a bulk copy that never lands) traps after 2^26 failed polls (seconds) instead of hanging
+// the GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     asm volatile(
         "{\n\t"
@@ -42,126 +42,115 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
-// ---- fences ----
+// shared-memory writes of the generic proxy (st.shared, cp.async) made visible to wgmma / TMA (async proxy)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// ---- tensor memory ----
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // same warp as alloc
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// 32 lanes x 32 consecutive columns -> 32 registers per thread (thread = lane of its warp's quadrant)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---- descriptors (cute/arch/mma_sm100_desc.hpp: SmemDescriptor / InstrDescriptor) ----
-// shared-memory matrix descriptor, no swizzle: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
-// version=1 [46,48) | layout_type=0 [61,64).  SBO = byte stride between core matrices along M/N,
-// LBO = byte stride between core matrices along K.
+// ---- wgmma (warpgroup MMA, sm_90a) ----
+// shared-memory matrix descriptor (cute/arch/mma_sm90_desc.hpp: GmmaDescriptor): start>>4 [0,14) | LBO>>4 [16,30) |
+// SBO>>4 [32,46) | base_offset [49,52) | layout_type [62,64) (0 = no swizzle, 1 = 128B swizzle).
+// No swizzle, K-major: SBO = byte stride between 8-row core matrices along N, LBO = byte stride between the two 16-byte
+// K chunks of one K = 8 step.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
-// instruction descriptor for kind::tf32, fp32 accumulate: c_format=F32 [4,6), a/b_format=TF32(2) [7,10)/[10,13),
-// a_major [15], b_major [16] (0 = K-major, 1 = MN-major), N>>3 [17,23), M>>4 [24,29)
-__device__ __forceinline__ uint32_t make_idesc_tf32(int m, int n, int a_mn_major, int b_mn_major) {
-    uint32_t d = 0;
-    d |= 1u << 4;
-    d |= 2u << 7;
-    d |= 2u << 10;
-    d |= (uint32_t)(a_mn_major & 1) << 15;
-    d |= (uint32_t)(b_mn_major & 1) << 16;
-    d |= (uint32_t)(n >> 3) << 17;
-    d |= (uint32_t)(m >> 4) << 24;
+// K-major tile written by TMA with CU_TENSOR_MAP_SWIZZLE_128B: rows of 128 bytes (one 32-float k-tile), 8-row swizzle
+// atoms of 1024 bytes (SBO); the tile base must be 1024-byte aligned; a K = 8 (32-byte) step advances the start address
+// by 32 bytes inside the atom.
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
+    d |= (uint64_t)1 << 16;             // LBO: unused for swizzled K-major operands
+    d |= (uint64_t)(1024u >> 4) << 32;  // SBO: next group of 8 rows
+    d |= (uint64_t)1 << 62;
     return d;
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// ---- operand tiles in shared memory (fp32 words, no swizzle) ----
-// Tile = ROWS (M or N extent, multiple of 8) x KT (=32) elements.
-//  K-major  : core matrix = 8 rows x 16 B; offset(r, k) = (r/8)*1024 + (k/4)*128 + (r%8)*16 + (k%4)*4
-//             -> SBO = 1024 (next 8 rows), LBO = 128 (next 16-byte K chunk); k8-step j starts at +256*j.
-//  MN-major : core matrix = 8 k x 16 B (4 consecutive m); offset(m, k) = (k/8)*(ROWS*32) + (m/4)*128 + (k%8)*16 + (m%4)*4
-//             -> SBO = 128 (next 4 m), LBO = ROWS*32 (next 8 k, unused by a K=8 instruction); k8-step j starts at +ROWS*32*j.
+// D[64 x N] += A[64 x 8] * B[N x 8]^T, fp32 accumulate: A from registers (the warpgroup's m64k8 tf32 fragment: warp w of
+// the group, lane l holds A[16 w + l/4 (+8)][l%4 (+4)] as a[0] = (r, k), a[1] = (r + 8, k), a[2] = (r, k + 4),
+// a[3] = (r + 8, k + 4)), B K-major in shared memory (descriptor).  d[i] (i < N / 2) is D[16 w + l/4 + 8 ((i/2) % 2)]
+// [8 (i/4) + 2 (l%4) + i%2].
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], const float *a, uint64_t bdesc);
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float (&d)[64], const float *a, uint64_t bdesc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, {%8, %9, %10, %11}, %12, p, 1, 1;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])), "l"(bdesc), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[64], const float *a, uint64_t bdesc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])), "l"(bdesc), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[64], const float *a, uint64_t bdesc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])), "l"(bdesc), "r"(1));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], const float *a, uint64_t bdesc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, {%64, %65, %66, %67}, %68, p, 1, 1;\n}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])), "l"(bdesc), "r"(1));
+}
+
+// ---- operand tiles in shared memory (fp32 words) ----
+// Tile = ROWS (N extent, multiple of 8) x KT (=32) elements, K-major, no swizzle: core matrix = 8 rows x 16 B;
+// offset(r, k) = (r/8)*1024 + (k/4)*128 + (r%8)*16 + (k%4)*4 -> SBO = 1024, LBO = 128; k8-step j starts at +256*j.
 constexpr int KT = 32;
 __host__ __device__ constexpr int b_tile_bytes(int bn) { return bn * KT * 4; }
 
-__device__ __forceinline__ uint32_t off_kmajor(int r, int k4) {  // k4 = k / 4 (one float4 per call)
-    return (uint32_t)((r >> 3) * 1024 + k4 * 128 + (r & 7) * 16);
-}
-__device__ __forceinline__ uint32_t off_mnmajor(int m4, int k, int rows) {  // m4 = m / 4
-    return (uint32_t)((k >> 3) * (rows * 32) + m4 * 128 + (k & 7) * 16);
-}
-
+__device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 __device__ __forceinline__ float4 tf32_lo(const float4 v) {
-    float4 r;
-    r.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-    r.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-    r.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-    r.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-    return r;
+    return make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w));
 }
-
-constexpr int TC_BM = 128;
-constexpr int TC_THREADS = 256;
-
-struct TcShared {  // micro-benchmark kernels of vk_tc_test.cu (tools/tc_fixed_cost.py)
-    uint64_t bar_stage[2];
-    uint64_t bar_done;
-    uint32_t tmem_base;
-};
-
-// Read the accumulator rows of this thread's TMEM quadrant: warp w owns lanes 32*(w%4)..+31; v receives 32
-// consecutive columns starting at `col`.
-__device__ __forceinline__ void tc_read_acc(const TcShared *sh, int col, float (&v)[32]) {
-    const int warp = threadIdx.x >> 5;
-    const uint32_t taddr = sh->tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)col;
-    tmem_ld32(taddr, v);
-}
-
-}  // namespace tc
-
-// =====================================================================================================
-// Layer GEMM main loop: operands are PLAIN K-major fp32 arrays in global memory, zero padded to 128 rows /
-// 32 columns with 16-byte aligned rows -- produced once per layer by the prep kernels (vk_vae.cu).  No
-// transform and no bounds checks on the way in; the tf32 remainders are derived in shared memory.
-namespace tc {
 
 struct OpRef {
     const float *hi, *lo;
@@ -177,12 +166,9 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 // ---- TMA: bulk tensor copies global -> shared, completion counted in bytes on an mbarrier ----
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 // box of the 2-D tensor map `tmap` at (c0 = innermost element, c1 = row) -> shared memory at smem_dst
 __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void *tmap, uint64_t *bar, int c0, int c1) {
@@ -191,148 +177,73 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void *tmap,
         "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-// shared-memory matrix descriptor of a K-major tile written by TMA with CU_TENSOR_MAP_SWIZZLE_128B: rows of 128 bytes
-// (one 32-float k-tile), 8-row swizzle atoms of 1024 bytes (SBO), layout_type = SWIZZLE_128B (2); the tile base must be
-// 1024-byte aligned; a K = 8 (32-byte) step advances the start address by 32 bytes inside the atom.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
-    d |= (uint64_t)1 << 16;                  // LBO: unused for swizzled K-major operands
-    d |= (uint64_t)(1024u >> 4) << 32;       // SBO: next group of 8 rows
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// 32 lanes x 16 consecutive columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// 32 lanes x 16 consecutive columns, registers -> tensor memory
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-        "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-        "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-        "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem, 128 lanes x 8 columns] * B[smem descriptor]^T
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
 
 // "Lane-major" storage of an A-role operand (the 128-row side of the GEMM): 128-row panels of an
 // [rows][ld] array, each k-tile of a panel is one 16 KB block  [k / 4 (8)][row (128)][k % 4 (4)]  so that
-// the 32 lanes of a warp read / write consecutive float4.  Same footprint as the row-major array.
+// consecutive rows are consecutive float4 for the producers, and the eight rows x four k of one wgmma fragment
+// register are 128 contiguous bytes for the main loop.  Same footprint as the row-major array.
 __host__ __device__ __forceinline__ size_t lane_major_index(int r, int k, int ld) {
     return (size_t)(r >> 7) * 128 * ld + (size_t)(k >> 5) * 4096 + (size_t)((k & 31) >> 2) * 512 + (size_t)(r & 127) * 4 + (k & 3);
 }
 
-// Warp-specialised pipeline.  A CTA is 8 producer/epilogue warps + 1 MMA warp (WS_THREADS = 288).
-// Shared memory bandwidth (128 B/clk) is what bounds a 3xTF32 tile loop that keeps both operands in shared
-// memory (each k-tile: copy in, read + write for the split, and twelve MMA reads of the 128-row operand), so
-// the 128-row operand A never touches shared memory:
-//   producers : warp w owns TMEM lanes 32 (w % 4).. and the k-half (w / 4) of each k-tile: it loads its 16
-//               values per row from the lane-major array (coalesced float4), splits them into the tf32 value
-//               ("hi" = the fp32 word, the MMA ignores the low mantissa bits) and the remainder ("lo") in
-//               registers and writes both to the A stage in TENSOR memory (tcgen05.st); the narrow operand
-//               B goes global -> shared with cp.async, each thread deriving "lo" of the chunk it copied;
-//               then proxy/tcgen05 fences and one arrival per warp on full[stage];
-//   MMA warp  : one lane waits full[stage], issues the 12 tcgen05.mma (A from tensor memory, B from shared
-//               memory; small terms first) of the k-tile and commits them to empty[stage].
-// Tensor memory: columns [0, 128) accumulator, then S stages of 64 columns (A_hi 32 | A_lo 32).
-// A stage is refilled once the MMAs that read it have completed; two tiles are in flight.
-constexpr int WS_THREADS = 288;
+// Main loop of the layer GEMMs.  A CTA is two warpgroups (WS_THREADS = 256); warpgroup g computes rows
+// [64 g, 64 g + 64) of the 128-row tile with one wgmma chain, its accumulator in registers.
+//   A (128-row operand): each thread loads its wgmma fragment of a k-tile straight from the lane-major array into
+//     registers (coalesced 128-byte rows, PA tiles in flight), the fp32 word serving as tf32 "hi" and the remainder
+//     "lo" derived in registers -- A never touches shared memory;
+//   B (narrow operand): a ring of WS_STAGES shared-memory stages [hi tile | lo tile] filled PB tiles ahead, either with
+//     cp.async by all threads (each deriving "lo" of the chunk it copied) or, TMA_B, by one thread through two bulk
+//     tensor copies (the weights and their tf32 remainders, pre-split once per step by prep_weights);
+//   per k-tile: one block barrier (the stage is complete; every warpgroup is done with the stage refilled next), then
+//     12 wgmma per warpgroup (4 K = 8 steps x {lo x hi, hi x lo, hi x hi}: small terms first), committed as one group
+//     that is waited for one k-tile later, so the tensor core runs while the next tile's barrier and split happen.
+// Runtime widths bn are computed with the next wgmma width N in {16, 32, 64, 128}; the columns past bn read stale ring
+// rows and are discarded by the epilogue.
+constexpr int WS_THREADS = 256;
 constexpr int WS_EPI_THREADS = 256;
-constexpr int WS_STAGES = 4;
-constexpr uint32_t WS_TMEM_COLS = 512;  // 128 + 4 * 64 rounded up to a power of two
-__host__ __device__ constexpr int ws_smem_bytes(int bn) { return WS_STAGES * 2 * b_tile_bytes(bn) + 1024; }  // bn = slot rows
+constexpr int WS_STAGES = 5;
+__host__ __device__ constexpr int wg_n(int bn) { return bn <= 16 ? 16 : (bn <= 32 ? 32 : (bn <= 64 ? 64 : 128)); }
+// ring bytes for tiles up to bn columns (+ 1024 for the alignment of the dynamic shared memory base)
+__host__ __device__ constexpr int ws_smem_bytes(int bn) { return WS_STAGES * 2 * b_tile_bytes(wg_n(bn)) + 1024; }
 
 struct WsShared {
-    uint64_t full[WS_STAGES], empty[WS_STAGES], done;
-    uint64_t acc_full[2], acc_empty[2];  // FLUSH: hand-over of the two alternating accumulators
-    uint32_t tmem_base;
+    uint64_t full[WS_STAGES];  // TMA_B: bytes of stage s landed
 };
 
-// FLUSH (wgrad: the reduction runs over the batch, hundreds of rows): the tensor core's fp32 accumulator TRUNCATES on
-// every accumulation, so the error of a long chain grows linearly with its length and is biased.  With FLUSH the chain
-// is cut every WS_FLUSH_KT k-tiles (128 batch rows): the MMA warp alternates between two accumulators in tensor memory
-// (columns [0, 128) and [384, 512)), and the epilogue warps add each finished group into fp32 REGISTERS (round to
-// nearest) while the next group accumulates -- `racc[i][j]` = column 32 i + 16 (warp / 4) + j of this thread's row.
+// The accumulator of one thread: d[i] as in wgmma_tf32, rows of its warpgroup's half of the tile.
+struct WsAcc {
+    float d[64];
+};
+
+// FLUSH (wgrad: the reduction runs over the batch, hundreds of rows): the chain of tensor-core accumulations is cut
+// every WS_FLUSH_KT k-tiles (128 batch rows), and each finished group is added into separate fp32 registers (round to
+// nearest), so that the error of a long chain stops growing with its length.
 constexpr int WS_FLUSH_KT = 4;
-constexpr int WS_DRAIN_LAG = 2;  // a group is drained once the producers are this many k-tiles into the next one
-constexpr uint32_t WS_ACC1_COL = 384u;
 
-// Stacked B: the tf32 remainder tile of B lies directly behind its hi tile in every ring stage, with the same layout, so
-// ONE MMA with N' = 2 bn rows of B computes A_hi x B_hi (accumulator columns [0, bn)) and A_hi x B_lo (columns
-// [bn, 2 bn)); a second one adds A_lo x B_hi into [0, bn); the epilogue adds the two column ranges.  A k-step is then 2
-// tcgen05.mma instead of 3 -- and an MMA with M = 128 costs the issuing thread ~47 cycles for any N <= 64 (64 cycles at
-// N = 128; tools/tc_fixed_cost.py, also with alternating accumulators: an issue cost, not a dependency), which is what
-// bounds the main loop of the narrow tiles small batches use.  Needs 2 bn <= 128 accumulator columns, a single
-// accumulator (no FLUSH) and, with TMA boxes of slot_rows rows, a full tile (bn == slot_rows).
-constexpr bool WS_STACK_B = true;
-template <bool TMA_B, bool FLUSH>
-__device__ __forceinline__ bool ws_stacked(int bn, int slot_rows) {
-    return WS_STACK_B && !FLUSH && 2 * bn <= 128 && (!TMA_B || bn == slot_rows);
-}
-
-// D[128 x bn] = sum over k-tiles [kt0, kt0 + nk) of A[m0.., k] * B[n0.., k]^T.  A: lane-major (m0 a multiple
-// of 128), B: plain K-major; both fp32, zero padded to whole tiles (ld = floats per row, multiple of 32).
-// Returns true for the 256 epilogue threads (accumulator complete), false for the MMA warp (which is done).
-//
-// TMA_B: the B operand (weights) is fetched by the TMA engine instead: one elected thread arms full[stage] with the
-// byte count and issues two bulk tensor copies (the fp32 tile and its pre-split tf32 remainder, written once per step by
-// prep_weights) through 128B-swizzled tensor maps whose box is 32 floats x `slot_rows` rows; the producer warps then
-// only feed A.  `slot_rows` (= the launch's tile width, >= bn) sizes the ring slots; tm_hi / tm_lo point to CUtensorMap
-// objects in kernel-parameter space (__grid_constant__).
-template <bool TMA_B = false, bool FLUSH = false>
-__device__ __forceinline__ bool ws_mainloop(const float *A, int lda, int m0, const float *B, int ldb, int n0, int bn,
-                                            int kt0, int nk, uint8_t *smem, WsShared *sh, int slot_rows = 0,
-                                            const void *tm_hi = nullptr, const void *tm_lo = nullptr,
-                                            float (*racc)[16] = nullptr) {
-    // PA: A tiles in flight as global loads into registers; PB: B tiles issued ahead into the shared-memory ring.
-    // A k-tile of A is 16 KB per CTA read from L2 with ~0.8 us of latency: two tiles in flight held the main loop to
-    // 0.43-0.47 us per k-tile (latency / 2) against the 0.29 us the 12 MMAs need (tools/kernel_timeline.py).
-    constexpr int S = WS_STAGES, PA = 4, PB = 3;
-    static_assert(PB < S && PA <= S, "ring depth");
+template <int N, bool TMA_B, bool FLUSH>
+__device__ __forceinline__ void ws_loop(const float *A, int lda, int m0, const float *B, int ldb, int n0, int bn, int kt0, int nk,
+                                        uint8_t *smem, WsShared *sh, int slot_rows, const void *tm_hi, const void *tm_lo,
+                                        float (&d)[64]) {
+    constexpr int S = WS_STAGES, PB = S - 2, PA = FLUSH ? 2 : 4;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int bbytes = b_tile_bytes(TMA_B ? slot_rows : bn), sbytes = 2 * bbytes;
+    // ring stage = [hi: R rows | lo: R rows]; TMA boxes are slot_rows rows, the wgmma reads N rows
+    const int R = TMA_B ? wg_n(slot_rows) : N;
+    const int bbytes = b_tile_bytes(R), sbytes = 2 * bbytes;
     const uint32_t smem_base = smem_u32(smem);
     // B chunk q = tid + 256 i of a tile: row ((q >> 6) << 3) | (q & 7) = r0 + 32 i, 16-byte column k4, at byte q * 16
     const int r0 = ((tid >> 6) << 3) | (tid & 7), k4 = (tid >> 3) & 7;
     const float *pb = B + (size_t)(n0 + r0) * ldb + (size_t)kt0 * KT + k4 * 4;
     const size_t b_step = (size_t)32 * ldb;
-    const int nbi = bn >> 5;                                // whole 32-row groups of the B tile
-    const bool b_tail = tid < (bn & 31) * 8;                // + 16 rows when bn is an odd multiple of 16
+    const int nbi = bn >> 5;                  // whole 32-row groups of the B tile
+    const bool b_tail = tid < (bn & 31) * 8;  // + 16 rows when bn is an odd multiple of 16
     const uint32_t soff = (uint32_t)tid * 16u;
-    // A: row 32 (warp % 4) + lane of the panel, float4 groups 4 (warp / 4) .. + 3 of each k-tile
-    const float4 *pa = reinterpret_cast<const float4 *>(A + (size_t)(m0 >> 7) * 128 * lda + (size_t)kt0 * 4096) +
-                       (warp >> 2) * 4 * 128 + (warp & 3) * 32 + lane;
+    // A: fragment rows r1 = 64 (warp / 4) + 16 (warp % 4) + lane / 4 and r1 + 8, k = 4 j + lane % 4 (j < 8)
+    const int r1 = 64 * (warp >> 2) + 16 * (warp & 3) + (lane >> 2);
+    const float *pa = A + (size_t)(m0 >> 7) * 128 * lda + (size_t)kt0 * 4096 + r1 * 4 + (lane & 3);
     auto issue_b = [&](int kt, int slot) {
         if (TMA_B) {
             if (tid == 0) {
-                mbar_expect_tx(&sh->full[slot], (uint32_t)sbytes);
+                mbar_arrive_expect_tx(&sh->full[slot], (uint32_t)(2 * b_tile_bytes(slot_rows)));
                 tma_load_2d(smem_base + slot * sbytes, tm_hi, &sh->full[slot], (kt0 + kt) * KT, n0);
                 tma_load_2d(smem_base + slot * sbytes + bbytes, tm_lo, &sh->full[slot], (kt0 + kt) * KT, n0);
             }
@@ -350,219 +261,132 @@ __device__ __forceinline__ bool ws_mainloop(const float *A, int lda, int m0, con
         if (b_tail)
             *reinterpret_cast<float4 *>(st + bbytes + nbi * 4096) = tf32_lo(*reinterpret_cast<const float4 *>(st + nbi * 4096));
     };
-    auto load_a = [&](int kt, float4 (&v)[4]) {
-        const float4 *g = pa + (size_t)kt * 1024;
+    // v[4 s .. 4 s + 3] = the fragment of K = 8 step s: (r1, 8s + l%4), (r1 + 8, ..), (r1, 8s + 4 + l%4), (r1 + 8, ..)
+    auto load_a = [&](int kt, float (&v)[16]) {
+        const float *g = pa + (size_t)kt * 4096;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) v[j] = __ldg(g + j * 128);
+        for (int j = 0; j < 8; ++j) {
+            v[2 * j] = __ldg(g + j * 512);
+            v[2 * j + 1] = __ldg(g + j * 512 + 32);
+        }
     };
-    // the first tiles are in flight while barriers / tensor memory are set up
-    float4 ra[PA][4];
-    if (warp < 8) {
+
+    float ra[PA][16], lo[2][16];
+    float racc[FLUSH ? 64 : 1];
+    if constexpr (FLUSH) {
 #pragma unroll
-        for (int t = 0; t < PB; ++t) {
-            if (t < nk && !TMA_B) issue_b(t, t);  // (the bulk copies need the barriers: issued after the set-up below)
-            if (!TMA_B) cp_async_commit();
-        }
-#pragma unroll
-        for (int t = 0; t < PA; ++t)
-            if (t < nk) load_a(t, ra[t]);
+        for (int i = 0; i < 64; ++i) racc[i] = 0.0f;
     }
-    if (tid == 0) {
+    if (TMA_B && tid == 0) {
 #pragma unroll
-        for (int s = 0; s < S; ++s) {
-            mbar_init(&sh->full[s], 8);
-            mbar_init(&sh->empty[s], 1);
-        }
-        mbar_init(&sh->done, 1);
-        if (FLUSH) {
-            mbar_init(&sh->acc_full[0], 1);
-            mbar_init(&sh->acc_full[1], 1);
-            mbar_init(&sh->acc_empty[0], 8);
-            mbar_init(&sh->acc_empty[1], 8);
-        }
+        for (int s = 0; s < S; ++s) mbar_init(&sh->full[s], 1);
         mbar_fence_init();
     }
-    if (warp == 0) tmem_alloc(&sh->tmem_base, WS_TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    tl_mark(8);
-    if (TMA_B && warp < 8) {
+    if (!TMA_B) {
 #pragma unroll
+        for (int t = 0; t < PB; ++t) {
+            if (t < nk) issue_b(t, t);
+            cp_async_commit();
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < PA; ++t)
+        if (t < nk) load_a(t, ra[t]);
+    __syncthreads();  // barriers initialised
+    if (TMA_B) {
         for (int t = 0; t < PB; ++t)
             if (t < nk) issue_b(t, t);
     }
-    const uint32_t tmem_d = sh->tmem_base;
-    if (warp == 8) {
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_tf32(TC_BM, bn, 0, 0);
-            const bool stk = ws_stacked<TMA_B, FLUSH>(bn, slot_rows);
-            const uint32_t idesc2 = make_idesc_tf32(TC_BM, 2 * bn, 0, 0);
-            const uint64_t desc0 = TMA_B ? make_smem_desc_sw128(smem_base) : make_smem_desc(smem_base, 128, 1024);
-            const uint32_t kstep = TMA_B ? 2u : 16u;  // start-address units (16 bytes) per K = 8 step
-            int slot = 0;
-            uint32_t phase = 0;
-            for (int kt = 0; kt < nk; ++kt) {
-                const int grp = FLUSH ? kt / WS_FLUSH_KT : 0;
-                const bool grp_first = FLUSH ? (kt % WS_FLUSH_KT == 0) : (kt == 0);
-                const bool grp_last = FLUSH ? ((kt + 1) % WS_FLUSH_KT == 0 || kt == nk - 1) : (kt == nk - 1);
-                const uint32_t tmem_acc = tmem_d + ((FLUSH && (grp & 1)) ? WS_ACC1_COL : 0u);
-                // the epilogue warps must have drained this accumulator's previous group (two groups ago)
-                if (FLUSH && grp_first && grp >= 2) mbar_wait(&sh->acc_empty[grp & 1], (uint32_t)(((grp >> 1) - 1) & 1));
-                mbar_wait(&sh->full[slot], phase);
-                tc_fence_after();
-                const uint32_t ah = tmem_d + 128u + 64u * slot, al = ah + 32u;
-                // descriptors differ only in the 14-bit start-address field: add (byte offset >> 4)
-                const uint64_t bh = desc0 + (uint64_t)((uint32_t)(slot * sbytes) >> 4);
-                const uint64_t bl = bh + (uint64_t)((uint32_t)bbytes >> 4);
-                if (stk) {
+    const uint64_t desc0 = TMA_B ? make_smem_desc_sw128(smem_base) : make_smem_desc(smem_base, 128, 1024);
+    const uint32_t kstep = TMA_B ? 2u : 16u;  // start-address units (16 bytes) per K = 8 step
+    for (int kb = 0; kb < nk; kb += PA) {
 #pragma unroll
-                    for (int j = 0; j < KT / 8; ++j) {
-                        umma_tf32_ts(tmem_acc, ah + 8u * j, bh + kstep * j, idesc2, (grp_first && j == 0) ? 0u : 1u);  // hi x [hi; lo]
-                        umma_tf32_ts(tmem_acc, al + 8u * j, bh + kstep * j, idesc, 1u);                                // lo x hi
+        for (int i = 0; i < PA; ++i) {
+            const int kt = kb + i;
+            if (kt >= nk) break;
+            const int slot = kt % S;
+            if (TMA_B) {
+                mbar_wait(&sh->full[slot], (uint32_t)((kt / S) & 1));
+            } else {
+                cp_async_wait<PB - 1>();  // this thread's copies of tile kt have landed (one group per tile)
+                split_b(slot);
+                fence_async_smem();
+            }
+            // stage kt complete for everyone; every warpgroup has retired the wgmma of tile kt - 2 (waited for below),
+            // the last reader of the stage of tile kt + PB
+            __syncthreads();
+            if (kt + PB < nk) issue_b(kt + PB, (kt + PB) % S);
+            if (!TMA_B) cp_async_commit();
+            float(&hi)[16] = ra[i];
+            float(&l)[16] = lo[i & 1];
+#pragma unroll
+            for (int e = 0; e < 16; ++e) l[e] = tf32_lo(hi[e]);
+            const uint64_t bh = desc0 + (uint64_t)((uint32_t)(slot * sbytes) >> 4);
+            const uint64_t bl = bh + (uint64_t)((uint32_t)bbytes >> 4);
+            wgmma_fence();
+#pragma unroll
+            for (int s = 0; s < KT / 8; ++s) {
+                wgmma_tf32<N>(d, l + 4 * s, bh + kstep * s);
+                wgmma_tf32<N>(d, hi + 4 * s, bl + kstep * s);
+                wgmma_tf32<N>(d, hi + 4 * s, bh + kstep * s);
+            }
+            wgmma_commit();
+            if constexpr (FLUSH) {
+                if ((kt + 1) % WS_FLUSH_KT == 0 && kt != nk - 1) {
+                    wgmma_wait<0>();
+#pragma unroll
+                    for (int e = 0; e < N / 2; ++e) {
+                        racc[e] += d[e];
+                        d[e] = 0.0f;
                     }
                 } else {
-#pragma unroll
-                    for (int j = 0; j < KT / 8; ++j) {
-                        umma_tf32_ts(tmem_acc, al + 8u * j, bh + kstep * j, idesc, (grp_first && j == 0) ? 0u : 1u);  // small terms first
-                        umma_tf32_ts(tmem_acc, ah + 8u * j, bl + kstep * j, idesc, 1u);
-                        umma_tf32_ts(tmem_acc, ah + 8u * j, bh + kstep * j, idesc, 1u);
-                    }
+                    wgmma_wait<1>();
                 }
-                umma_commit(&sh->empty[slot]);
-                if (FLUSH && grp_last && kt != nk - 1) umma_commit(&sh->acc_full[grp & 1]);
-                if (kt == nk - 1) umma_commit(&sh->done);
-                if (++slot == S) {
-                    slot = 0;
-                    phase ^= 1u;
-                }
+            } else {
+                wgmma_wait<1>();  // tile kt - 1 retired: its A registers are free
             }
+            if (kt >= 1 && kt - 1 + PA < nk) load_a(kt - 1 + PA, ra[(i + PA - 1) % PA]);
         }
-        return false;
     }
-    const uint32_t a_lane = tmem_d + ((uint32_t)((warp & 3) * 32) << 16) + 128u + (uint32_t)(warp >> 2) * 16u;
-    auto produce = [&](int kt, float4(&v)[4]) {
-        const int slot = kt % S;
-        // A tile kt: registers -> tensor memory.  Its stage is free: every producer thread waited for the MMAs of tile
-        // kt - S before B of tile kt was issued (PB tiles ago, below).
-        float hi[16], lo[16];
+    wgmma_wait<0>();
+    if constexpr (FLUSH) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const float4 l4 = tf32_lo(v[j]);
-            hi[4 * j] = v[j].x; hi[4 * j + 1] = v[j].y; hi[4 * j + 2] = v[j].z; hi[4 * j + 3] = v[j].w;
-            lo[4 * j] = l4.x; lo[4 * j + 1] = l4.y; lo[4 * j + 2] = l4.z; lo[4 * j + 3] = l4.w;
-        }
-        tc_fence_after();
-        tmem_st16(a_lane + 64u * slot, hi);
-        tmem_st16(a_lane + 64u * slot + 32u, lo);
-        if (kt + PA < nk) load_a(kt + PA, v);  // v's registers are free again
-        if (!TMA_B) {
-            cp_async_wait<PB - 1>();  // this thread's B copies of tile kt have landed (one group per produced tile)
-            split_b(slot);
-        }
-        tmem_wait_st();
-        if (!TMA_B) fence_async_smem();  // shared-memory writes visible to the tensor core (async proxy)
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sh->full[slot]);
-        // B of tile kt + PB, AFTER this tile has been handed over: its stage was read by the MMAs of tile
-        // kt + PB - S (the previous tile for PB = S - 1), which run while the A part above is produced
-        const int nt = kt + PB;
-        if (nt < nk) {
-            if (nt >= S) mbar_wait(&sh->empty[nt % S], (uint32_t)(((nt / S) - 1) & 1));
-            issue_b(nt, nt % S);
-        }
-        if (!TMA_B) cp_async_commit();
-        if (kt < 20) tl_mark(10 + kt);
-    };
-    // FLUSH: add a finished group (all but the last, which the epilogue reads) into the register accumulators
-    int next_drain = 0;
-    auto drain_ready = [&](int kt_done) {  // after producing tile kt_done
-        if (!FLUSH) return;
-        while ((next_drain + 1) * WS_FLUSH_KT + WS_DRAIN_LAG <= kt_done + 1 && (next_drain + 1) * WS_FLUSH_KT < nk) {
-            const int a = next_drain & 1;
-            mbar_wait(&sh->acc_full[a], (uint32_t)((next_drain >> 1) & 1));
-            tc_fence_after();
-            const uint32_t base = tmem_d + ((uint32_t)((warp & 3) * 32) << 16) + (a ? WS_ACC1_COL : 0u);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int c = (warp >> 2) * 16 + 32 * i;
-                if (c < bn) {
-                    float v[16];
-                    tmem_ld16(base + (uint32_t)c, v);
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) racc[i][j] += v[j];
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sh->acc_empty[a]);
-            ++next_drain;
-        }
-    };
-    if (FLUSH) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 16; ++j) racc[i][j] = 0.0f;
+        for (int e = 0; e < N / 2; ++e) d[e] += racc[e];
     }
-    for (int kt = 0; kt < nk; kt += PA) {
-#pragma unroll
-        for (int i = 0; i < PA; ++i)
-            if (kt + i < nk) {
-                produce(kt + i, ra[i]);
-                drain_ready(kt + i);
-            }
-    }
-    if (FLUSH) {  // groups that completed inside the last WS_DRAIN_LAG tiles
-        while ((next_drain + 1) * WS_FLUSH_KT < nk) drain_ready(1 << 28);
-    }
-    tl_mark(9);
-    if (nk > 0) mbar_wait(&sh->done, 0);
-    tc_fence_after();
-    return true;
+    __syncthreads();  // every warpgroup is done with the ring: the caller may reuse the shared memory
 }
 
-// Accumulator -> shared tile [128][ts] (raw values): warp w owns TMEM lanes 32*(w%4)..+31, the two warp
-// groups take alternate 16-column chunks.  nk == 0 (an empty split) yields zeros.
-// racc != nullptr (FLUSH): the last group sits in accumulator ((nk - 1) / WS_FLUSH_KT) & 1 and the earlier groups in
-// the register sums of ws_mainloop.
-__device__ __forceinline__ void ws_acc_to_tile(const WsShared *sh, int bn, int nk, float *tile, int ts,
-                                               const float (*racc)[16] = nullptr, bool stacked = false) {
+// acc = A[m0.., k] * B[n0.., k]^T over k-tiles [kt0, kt0 + nk) (rows of this thread's warpgroup, see WsAcc).
+// A: lane-major (m0 a multiple of 128), B: plain K-major; both fp32, zero padded to whole tiles (ld = floats per
+// row, multiple of 32), B rows up to n0 + bn (bn a multiple of 16, <= 128).  nk == 0 (an empty split) yields zeros.
+// TMA_B: B through tm_hi / tm_lo, CUtensorMap objects in kernel-parameter space (__grid_constant__) of 128B-swizzled
+// boxes of 32 floats x slot_rows rows (slot_rows = the launch's tile width, >= bn).  All WS_THREADS threads call it.
+template <bool TMA_B = false, bool FLUSH = false>
+__device__ __forceinline__ void ws_mainloop(const float *A, int lda, int m0, const float *B, int ldb, int n0, int bn,
+                                            int kt0, int nk, uint8_t *smem, WsShared *sh, WsAcc &acc, int slot_rows = 0,
+                                            const void *tm_hi = nullptr, const void *tm_lo = nullptr) {
+#pragma unroll
+    for (int e = 0; e < 64; ++e) acc.d[e] = 0.0f;
+    switch (wg_n(bn)) {
+        case 16: ws_loop<16, TMA_B, FLUSH>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, sh, slot_rows, tm_hi, tm_lo, acc.d); break;
+        case 32: ws_loop<32, TMA_B, FLUSH>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, sh, slot_rows, tm_hi, tm_lo, acc.d); break;
+        case 64: ws_loop<64, TMA_B, FLUSH>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, sh, slot_rows, tm_hi, tm_lo, acc.d); break;
+        default: ws_loop<128, TMA_B, FLUSH>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, sh, slot_rows, tm_hi, tm_lo, acc.d); break;
+    }
+}
+
+// Accumulator -> shared tile [128][ts] (raw values), columns < bn.
+__device__ __forceinline__ void ws_acc_to_tile(const WsAcc &acc, int bn, float *tile, int ts) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t acc_col = (racc && nk > 0 && (((nk - 1) / WS_FLUSH_KT) & 1)) ? WS_ACC1_COL : 0u;
+    const int row = 64 * (warp >> 2) + 16 * (warp & 3) + (lane >> 2), col = 2 * (lane & 3);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int c = (warp >> 2) * 16 + 32 * i;
-        if (c >= bn) break;
-        float v[16];
-        if (nk > 0) tmem_ld16(sh->tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + acc_col + (uint32_t)c, v);
-        else
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = 0.0f;
-        if (racc) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] += racc[i][j];
-        }
-        if (stacked && nk > 0) {  // + A_hi x B_lo, accumulated in the columns behind the tile's own (ws_stacked)
-            float w[16];
-            tmem_ld16(sh->tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(bn + c), w);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] += w[j];
-        }
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4)
-            *reinterpret_cast<float4 *>(tile + row * ts + c + 4 * j4) =
-                make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
+    for (int i = 0; i < 64; i += 2) {
+        const int c = 8 * (i >> 2) + col, r = row + 8 * ((i >> 1) & 1);
+        if (c < bn) *reinterpret_cast<float2 *>(tile + r * ts + c) = make_float2(acc.d[i], acc.d[i + 1]);
     }
 }
 
-// all epilogue threads: tile complete for everyone, tensor memory released
-__device__ __forceinline__ void ws_tile_end(WsShared *sh) {
-    tc_fence_before();
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 0) tmem_dealloc(sh->tmem_base, WS_TMEM_COLS);
-}
+// all threads: the tile in shared memory is complete for everyone
+__device__ __forceinline__ void ws_tile_end() { __syncthreads(); }
 
 }  // namespace tc

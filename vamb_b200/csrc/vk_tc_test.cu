@@ -1,4 +1,4 @@
-// Stand-alone check of the production tcgen05 3xTF32 main loop (tc::ws_mainloop, vk_tc.cuh): C[M, N] = A * B^T on
+// Stand-alone check of the production wgmma 3xTF32 main loop (tc::ws_mainloop, vk_tc.cuh): C[M, N] = A * B^T on
 // staged operands, every tile width and split-K offsets.  Used by tests/test_tc_gpu.py.
 #include "vk_tc.cuh"
 
@@ -21,17 +21,14 @@ ws_gemm_test_kernel(const float *A, int lda, const float *B, int ldb, float *C, 
     const int m0 = blockIdx.y * 128, n0 = blockIdx.x * tile_n;
     int bn = N - n0;
     bn = bn > tile_n ? tile_n : ((bn + 15) & ~15);
-    float racc[4][16];
-    const bool alive =
-        tm.flush ? tc::ws_mainloop<false, true>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, &sh, 0, nullptr, nullptr, racc)
-        : tm.use_tma ? tc::ws_mainloop<true>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, &sh, tile_n, &tm.hi, &tm.lo)
-                     : tc::ws_mainloop<false>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, &sh);
-    if (!alive) return;
+    tc::WsAcc acc;
+    if (tm.flush) tc::ws_mainloop<false, true>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, &sh, acc);
+    else if (tm.use_tma) tc::ws_mainloop<true>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, &sh, acc, tile_n, &tm.hi, &tm.lo);
+    else tc::ws_mainloop<false>(A, lda, m0, B, ldb, n0, bn, kt0, nk, smem, &sh, acc);
     constexpr int TS = 132;
     float *tile = reinterpret_cast<float *>(smem);
-    if (tm.flush) tc::ws_acc_to_tile(&sh, bn, nk, tile, TS, racc);
-    else tc::ws_acc_to_tile(&sh, bn, nk, tile, TS, nullptr, tm.use_tma ? tc::ws_stacked<true, false>(bn, tile_n) : tc::ws_stacked<false, false>(bn, 0));
-    tc::ws_tile_end(&sh);
+    tc::ws_acc_to_tile(acc, bn, tile, TS);
+    tc::ws_tile_end();
     for (int q = threadIdx.x; q < 128 * bn; q += tc::WS_EPI_THREADS) {
         const int r = q / bn, c = q - r * bn;
         if (m0 + r < M && n0 + c < N) C[(int64_t)(m0 + r) * N + n0 + c] = tile[r * TS + c];
@@ -43,7 +40,7 @@ ws_gemm_test_kernel(const float *A, int lda, const float *B, int ldb, float *C, 
 // A_lane: [ceil(M / 128) * 128 rows, lda] in tc::lane_major_index order; B: [ceil(N / tile_n) * tile_n rows, ldb]
 // row-major; lda, ldb multiples of 32 covering k-tiles [0, kt0 + nk).  tile_n: multiple of 16 in [16, 128].
 // B_lo != NULL: B through TMA (B_lo = the tf32 remainders of B, same shape), as the forward / dgrad GEMMs fetch weights.
-// flush != 0 (with B_lo == NULL): the wgrad variant -- accumulation chain cut every 4 k-tiles (two accumulators).
+// flush != 0 (with B_lo == NULL): the wgrad variant -- accumulation chain cut every 4 k-tiles.
 extern "C" int vk_tc_gemm_test(const float *A_lane, int lda, const float *B, const float *B_lo, int ldb, float *C, int M, int N,
                                int tile_n, int kt0, int nk, int flush, void *stream) {
     cudaStream_t s = (cudaStream_t)stream;
@@ -64,129 +61,6 @@ extern "C" int vk_tc_gemm_test(const float *A_lane, int lda, const float *B, con
         if (vk_make_tmap_2d(&tm.hi, B, ldb, rows, tile_n) || vk_make_tmap_2d(&tm.lo, B_lo, ldb, rows, tile_n)) return 1;
     }
     ws_gemm_test_kernel<<<grid, tc::WS_THREADS, smem, s>>>(A_lane, lda, B, ldb, C, M, N, tile_n, kt0, nk, tm);
-    VK_LAUNCH_CHECK();
-    return 0;
-}
-
-// ---- launch / prologue overhead probes (tools/tc_fixed_cost.py) ----
-namespace {
-// mode 0: nothing; 1: + barrier init + TMEM alloc/dealloc; 2: + one MMA + commit + wait; 3: + __threadfence + atomic
-__global__ void __launch_bounds__(tc::TC_THREADS, 1) tc_overhead_kernel(int mode, int *counter) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ tc::TcShared sh;
-    if (mode == 0) return;
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    if (tid == 0) {
-        tc::mbar_init(&sh.bar_done, 1);
-        tc::mbar_fence_init();
-    }
-    if (warp == 0) tc::tmem_alloc(&sh.tmem_base, 128);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    if (mode >= 2) {
-        for (int i = tid; i < 16384; i += tc::TC_THREADS) reinterpret_cast<float *>(smem)[i] = 1.0f;
-        tc::fence_async_smem();
-        __syncthreads();
-        if (tid == 0) {
-            const uint64_t d = tc::make_smem_desc(tc::smem_u32(smem), 128, 1024);
-            tc::umma_tf32(sh.tmem_base, d, d + (32768 >> 4), tc::make_idesc_tf32(128, 32, 0, 0), 0u);
-            tc::umma_commit(&sh.bar_done);
-        }
-        tc::mbar_wait(&sh.bar_done, 0);
-        tc::tc_fence_after();
-    }
-    if (mode == 3) {
-        __syncthreads();
-        if (tid == 0) {
-            __threadfence();
-            atomicAdd(counter, 1);
-        }
-    }
-    if (mode == 4) {  // + accumulator read-back and a global store
-        float v[32];
-        tc::tc_read_acc(&sh, 0, v);
-        float t = 0.f;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) t += v[j];
-        if (t == 123.456f) counter[1] = 1;
-    }
-    if (mode == 5) {  // sixteen dependent MMA+commit+wait round trips instead of one
-        for (int it = 1; it < 16; ++it) {
-            if (tid == 0) {
-                const uint64_t d = tc::make_smem_desc(tc::smem_u32(smem), 128, 1024);
-                tc::umma_tf32(sh.tmem_base, d, d + (32768 >> 4), tc::make_idesc_tf32(128, 32, 0, 0), 1u);
-                tc::umma_commit(&sh.bar_done);
-            }
-            tc::mbar_wait(&sh.bar_done, (uint32_t)(it & 1));
-            tc::tc_fence_after();
-        }
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(sh.tmem_base, 128);
-}
-}  // namespace
-
-extern "C" int vk_tc_overhead_test(int mode, int grid, int smem_bytes, int *counter, void *stream) {
-    static bool attr = false;
-    if (!attr) {
-        VK_CUDA(cudaFuncSetAttribute(tc_overhead_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr = true;
-    }
-    tc_overhead_kernel<<<grid, tc::TC_THREADS, smem_bytes, (cudaStream_t)stream>>>(mode, counter);
-    VK_LAUNCH_CHECK();
-    return 0;
-}
-
-// ---- issue / execution rate of back-to-back tcgen05.mma (tools/tc_fixed_cost.py) ----
-namespace {
-__global__ void __launch_bounds__(tc::TC_THREADS, 1) tc_mma_rate_kernel(int n_mma, int n, int swizzle, long long *out) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ tc::TcShared sh;
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    if (tid == 0) {
-        tc::mbar_init(&sh.bar_done, 1);
-        tc::mbar_fence_init();
-    }
-    if (warp == 0) tc::tmem_alloc(&sh.tmem_base, 256);
-    for (int i = tid; i < 16384; i += tc::TC_THREADS) reinterpret_cast<float *>(smem)[i] = 1.0f;
-    tc::fence_async_smem();
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    if (tid == 0) {
-        uint64_t d = tc::make_smem_desc(tc::smem_u32(smem), swizzle ? 16 : 128, 1024);
-        if (swizzle) d |= (uint64_t)2 << 61;  // SWIZZLE_128B (modes 1, 2, 3)
-        const uint64_t da = d, db = d + (32768 >> 4);
-        const uint32_t idesc = tc::make_idesc_tf32(128, n, 0, 0);
-        const long long t0 = clock64();
-        if (swizzle == 2)  // A operand from tensor memory (columns 128..), B from shared memory
-            for (int i = 0; i < n_mma; ++i) tc::umma_tf32_ts(sh.tmem_base, sh.tmem_base + 128u + 8u * (i & 3), db, idesc, 1u);
-        else if (swizzle == 3)  // as 2, successive MMAs into two DIFFERENT accumulators (n <= 64): is the per-MMA cost a
-                                // dependency on the accumulator or an issue cost?
-            for (int i = 0; i < n_mma; ++i)
-                tc::umma_tf32_ts(sh.tmem_base + ((i & 1) ? 192u : 0u), sh.tmem_base + 128u + 8u * (i & 3), db, idesc, 1u);
-        else
-            for (int i = 0; i < n_mma; ++i) tc::umma_tf32(sh.tmem_base, da + (uint64_t)((i & 3) * (swizzle ? 2 : 16)), db, idesc, 1u);
-        tc::umma_commit(&sh.bar_done);
-        const long long t1 = clock64();
-        tc::mbar_wait(&sh.bar_done, 0);
-        const long long t2 = clock64();
-        out[0] = t1 - t0;
-        out[1] = t2 - t0;
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(sh.tmem_base, 256);
-}
-}  // namespace
-
-extern "C" int vk_tc_mma_rate_test(int n_mma, int n, int swizzle, long long *out_dev, void *stream) {
-    VK_CUDA(cudaFuncSetAttribute(tc_mma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    tc_mma_rate_kernel<<<1, tc::TC_THREADS, 100 * 1024, (cudaStream_t)stream>>>(n_mma, n, swizzle, out_dev);
     VK_LAUNCH_CHECK();
     return 0;
 }

@@ -1,4 +1,4 @@
-// vamb_b200 VAE kernels, fp32 CUDA-core path (sm_100a).
+// vamb_b200 VAE kernels, fp32 CUDA-core path (sm_90a).
 //
 // One optimiser step of vamb/encode.py (VAE.trainepoch :401-419) = 15 stream-ordered launches:
 //   batch_rows  | fwd x (2L+2) | loss | bwd x (2L+2) (wgrad + dgrad tiles in ONE grid) | dadapt
@@ -10,8 +10,8 @@
 //     its two batch reductions (sum dH, sum dH*Phat) are column sums of the dgrad epilogue.
 //   * bias gradients come out of the wgrad GEMM through a virtual all-ones input column.
 // All reductions are two-stage with a fixed order (no floating-point atomics): same inputs ->
-// same bits.  This file is the exact-fp32 reference path; vk_vae_tc.cu (tcgen05, 3xTF32) replaces
-// the GEMM core for large batches.
+// same bits.  The fp32 CUDA-core kernels below are the exact-fp32 path; the tensor-core kernels (wgmma, 3xTF32,
+// vk_tc.cuh) replace the GEMM core for large batches.
 //
 // Reference lines (RasmussenLab/vamb): encode.py:259-273 _encode, :276-286 reparameterize,
 // :288-304 _decode, :316-357 calc_loss, :442-484 encode; dadaptation==3.2 DAdaptAdam.step.
@@ -146,7 +146,7 @@ batch_rows_kernel(int64_t *batch_rows, const int64_t *batch_idx, const float *we
 // ------------------------------------------------------------------ operand loaders
 // at(r, c): element (row r, column c) of the logical [rows, cols] operand, 0 outside.
 // ld4(r, c4): elements (r, 4*c4 .. 4*c4+3) -- one 16-byte load per array when the row is 16-byte
-// aligned and fully inside, else four at() calls (used by the tcgen05 path, vk_tc.cuh).
+// aligned and fully inside, else four at() calls (used by the tensor-core path, vk_tc.cuh).
 __device__ __forceinline__ bool vec_ok(const void *p, int ld) {
     return ((ld & 3) == 0) && ((reinterpret_cast<uintptr_t>(p) & 15) == 0);
 }
@@ -726,9 +726,9 @@ __global__ void __launch_bounds__(GT) bwd_layer_kernel(BwdArgs a) {
     bn_backward_finalize(a, blockDim.x);
 }
 
-// ------------------------------------------------------------------ tcgen05 (3xTF32) layer kernels
+// ------------------------------------------------------------------ tensor-core (wgmma, 3xTF32) layer kernels
 // Same arguments and results as fwd_layer_kernel / bwd_layer_kernel; the GEMM core is the 128 x bn
-// tensor-core tile of vk_tc.cuh and the epilogue goes TMEM -> registers -> shared tile -> global.
+// tensor-core tile of vk_tc.cuh and the epilogue goes registers -> shared tile -> global.
 constexpr int TS = 132;  // padded row stride (floats) of the shared epilogue tile: conflict-free float4 rows
 
 __device__ __forceinline__ uint8_t *align1024(uint8_t *p) {
@@ -738,8 +738,8 @@ __device__ __forceinline__ uint8_t *align1024(uint8_t *p) {
 // Column sums of two per-element quantities over the 128 rows of the shared tile(s), in a fixed order, by ALL 256
 // epilogue threads: the tile's bn columns (a multiple of 16) are covered by G = 256 / bnp row groups (bnp = bn rounded
 // up to a power of two), thread (g, col) sums rows [g * 128 / G, (g + 1) * 128 / G) in double, and thread col folds the
-// G partials in order.  (One thread per column and half -- 64 serial double additions -- cost 1.65 us per layer at
-// B = 256, where only 32 of the 256 threads had a column: tools/kernel_timeline.py.)
+// G partials in order.  (One thread per column would leave most threads idle at small bn: 64 serial double additions
+// per column.)
 // f(r, c) -> (v0, v1).  Writes out0/out1[n0 + c] for c < bn with n0 + c < N.  s_cs: 512 doubles of shared memory.
 template <class F>
 __device__ __forceinline__ void tc_colsum2(int bn, int n0, int N, double (*s_cs)[2][128], double *out0, double *out1,
@@ -777,9 +777,9 @@ __device__ __forceinline__ void tc_colsum2(int bn, int n0, int N, double (*s_cs)
 }
 
 // ---- cluster fold: BatchNorm sums exchanged through distributed shared memory ----
-// When the row tiles of one column tile are a small thread-block cluster (B <= 512: 2 or 4 CTAs), the per-row-tile
+// When the row tiles of one column tile are a small thread-block cluster (B <= 256: 2 CTAs), the per-row-tile
 // column sums never leave the SMs: every CTA leaves its two sums per column in shared memory, one hardware cluster
-// barrier replaces the software grid barrier (global atomics + polling: 2-3 us per layer, tools/kernel_timeline.py),
+// barrier replaces the software grid barrier (global atomics + polling),
 // and every CTA reads its peers' sums with ld.shared::cluster in the SAME order as the global fold below (identical
 // doubles, identical results).  A second barrier before exit keeps the shared memory alive while peers read it.
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
@@ -930,9 +930,8 @@ struct BwdTcExtra {
 // LeakyReLU, dropout (one Philox call per four outputs) / the reparameterisation, and the global stores;
 // hidden layers in training add the BatchNorm column sums and the last CTA folds them.
 // TMA: the weight operand through cp.async.bulk.tensor; FLUSH: accumulation chain cut every 128 K-elements (fp32 register
-// sums, vk_tc.cuh) -- used for evaluation (`encode`), where the latent must stay within 1e-4 of fp32: the tensor core's
-// truncating accumulator alone leaves ~1e-5 of the accumulator magnitude per 512-deep layer (1.5e-4 on |mu| <= 11.5,
-// profiles/r02_encode_error.txt).  One instantiation per combination keeps every kernel's code (and its cold
+// sums, vk_tc.cuh) -- used for evaluation (`encode`), where the latent must stay within 1e-4 of fp32 whatever the
+// depth of the layer: a shorter accumulation chain on the tensor core bounds its rounding error.  One instantiation per combination keeps every kernel's code (and its cold
 // instruction-cache footprint at launch) to the path it runs.
 template <bool TMA, bool FLUSH>
 __global__ void __launch_bounds__(tc::WS_THREADS, 1) fwd_layer_tc_kernel(const __grid_constant__ FwdArgs a) {
@@ -953,15 +952,14 @@ __global__ void __launch_bounds__(tc::WS_THREADS, 1) fwd_layer_tc_kernel(const _
     const uint32_t k0 = (uint32_t)a.ctl->seed, k1 = (uint32_t)(a.ctl->seed >> 32);
     const uint32_t step_lo = (uint32_t)a.ctl->step, step_hi = (uint32_t)(a.ctl->step >> 32);
     const int nk = (a.K + tc::KT - 1) / tc::KT;
-    float racc[FLUSH ? 4 : 1][16];
-    if (!tc::ws_mainloop<TMA, FLUSH>(a.a_op.hi, a.a_op.ld, m0, a.b_op.hi, a.b_op.ld, n0, bn, 0, nk, smem, &sh, a.tile_n,
-                                     &a.tm_b_hi, &a.tm_b_lo, FLUSH ? racc : nullptr))
-        return;
+    tc::WsAcc acc;
+    tc::ws_mainloop<TMA, FLUSH>(a.a_op.hi, a.a_op.ld, m0, a.b_op.hi, a.b_op.ld, n0, bn, 0, nk, smem, &sh, acc, a.tile_n,
+                                &a.tm_b_hi, &a.tm_b_lo);
     tl_mark(2);
     float *tile = reinterpret_cast<float *>(smem);  // [128][TS]; the operand stages are dead now
-    tc::ws_acc_to_tile(&sh, bn, nk, tile, TS, FLUSH ? racc : nullptr, tc::ws_stacked<TMA, FLUSH>(bn, a.tile_n));
+    tc::ws_acc_to_tile(acc, bn, tile, TS);
     tl_mark(3);
-    tc::ws_tile_end(&sh);
+    tc::ws_tile_end();
     tl_mark(44);
 
     const bool hidden = a.kind == VK_LAYER_HIDDEN, is_mu = a.kind == VK_LAYER_MU;
@@ -974,7 +972,7 @@ __global__ void __launch_bounds__(tc::WS_THREADS, 1) fwd_layer_tc_kernel(const _
     // Lean pass for the case that carries the training run -- a hidden layer in training mode with on-device dropout, a
     // tile that lies fully inside [.., N) and a power-of-two tile width: the general loop below spends ~700 SASS
     // instructions per four outputs (64-bit address arithmetic for five optional outputs, per-element bounds, two inlined
-    // Philox bodies, an integer division; ncu: 11 of the 33 us of a 512 -> 512 layer at B = 4096), this one ~150.  Same
+    // Philox bodies, an integer division), this one ~150.  Same
     // values, same Philox stream: the keep test (float)(x >> 8) + 1) * 2^-24 > p is the integer test (x >> 8) >= floor(p 2^24).
     const bool lean = hidden && a.training && a.keep == nullptr && vec && (n0 + bn <= a.N) && ((q_per_row & (q_per_row - 1)) == 0);
     if (lean) {
@@ -1194,14 +1192,12 @@ __global__ void __launch_bounds__(tc::WS_THREADS, 1) bwd_layer_tc_kernel(const _
         int nb = a.B - b0;
         nb = nb < 0 ? 0 : (nb > x.k_per_split ? x.k_per_split : nb);
         const int nk = (nb + tc::KT - 1) / tc::KT;  // b0 is a multiple of 32; the staged operands are zero padded
-        float racc[FLUSH ? 4 : 1][16];
-        if (!tc::ws_mainloop<false, FLUSH>(a.wg_a.hi, a.wg_a.ld, m0, a.wg_b.hi, a.wg_b.ld, n0, bn, b0 / tc::KT, nk, smem, &sh, 0,
-                                           nullptr, nullptr, FLUSH ? racc : nullptr))
-            return;
+        tc::WsAcc acc;
+        tc::ws_mainloop<false, FLUSH>(a.wg_a.hi, a.wg_a.ld, m0, a.wg_b.hi, a.wg_b.ld, n0, bn, b0 / tc::KT, nk, smem, &sh, acc);
         tl_mark(2);
-        tc::ws_acc_to_tile(&sh, bn, nk, tile, TS, FLUSH ? racc : nullptr, tc::ws_stacked<false, FLUSH>(bn, 0));
+        tc::ws_acc_to_tile(acc, bn, tile, TS);
         tl_mark(3);
-        tc::ws_tile_end(&sh);
+        tc::ws_tile_end();
         float *gW = a.gW + (int64_t)split * x.slab, *gb = a.gb + (int64_t)split * x.slab;
         for (int q = tid; q < 128 * bn; q += tc::WS_EPI_THREADS) {
             const int r = q / bn, c = q - r * bn;
@@ -1226,9 +1222,9 @@ __global__ void __launch_bounds__(tc::WS_THREADS, 1) bwd_layer_tc_kernel(const _
     bn = bn > a.tile_n ? a.tile_n : ((bn + 15) & ~15);
     const float gsc = (float)(a.ctl->wbar / (double)a.B);
     const int nk = (a.N + tc::KT - 1) / tc::KT;
-    if (!tc::ws_mainloop<TMA, false>(a.dg_a.hi, a.dg_a.ld, m0, a.dg_b.hi, a.dg_b.ld, n0, bn, 0, nk, smem, &sh, a.tile_n,
-                                     &a.tm_dg_hi, &a.tm_dg_lo))
-        return;
+    tc::WsAcc acc;
+    tc::ws_mainloop<TMA, false>(a.dg_a.hi, a.dg_a.ld, m0, a.dg_b.hi, a.dg_b.ld, n0, bn, 0, nk, smem, &sh, acc, a.tile_n,
+                                &a.tm_dg_hi, &a.tm_dg_lo);
     TLD(2);
     const int q_per_row = bn >> 2;
     float *ptile = tile + 128 * TS;  // the previous layer's output P for the same rows / columns (zeros outside)
@@ -1268,8 +1264,8 @@ __global__ void __launch_bounds__(tc::WS_THREADS, 1) bwd_layer_tc_kernel(const _
             *reinterpret_cast<float4 *>(ptile + r * TS + c) = pv;
         }
     }
-    tc::ws_acc_to_tile(&sh, bn, nk, tile, TS, nullptr, tc::ws_stacked<TMA, false>(bn, a.tile_n));
-    tc::ws_tile_end(&sh);
+    tc::ws_acc_to_tile(acc, bn, tile, TS);
+    tc::ws_tile_end();
     TLD(3);
     const bool vec = ((a.K & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.d_in) & 15) == 0);
     const bool add_kld = a.in_kind == VK_IN_Z;
@@ -1808,7 +1804,10 @@ static int tc_nsplit(const vk_vae *net, int B) {
     return ns;
 }
 
-// output columns per CTA: narrower tiles for small batches so that enough CTAs exist
+// output columns per CTA: narrower tiles for small batches so that enough CTAs exist.  Chosen on an H100 SXM (400 W
+// power limit) with tools/train_speed.py, us per step with every width forced: B = 256: 16 -> 193, 32 -> 212;
+// B = 512: 32 -> 258, 64 -> 281; B = 1024: 32 / 64 -> 318 / 320; B = 2048: 64 -> 435, 128 -> 454; B = 4096: 128 -> 638,
+// 64 -> 702.
 static int tc_tile_n(int B) {
     static const int forced = env_int("VK_TC_TILE_N");  // tuning / debugging override
     if (forced >= 16 && forced <= 128 && (forced & 15) == 0) return forced;
@@ -1819,7 +1818,7 @@ static int tc_wg_tile_n(int B) {
     static const int forced = env_int("VK_TC_WG_TILE_N");
     if (forced >= 16 && forced <= 128 && (forced & 15) == 0) return forced;
     const int t = tc_tile_n(B);
-    return t < 32 ? 32 : t;  // measured: 32 for B <= 1024, the dgrad width above (tools/train_speed.py)
+    return t < 32 ? 32 : t;  // 32 for B <= 1024, the dgrad width above (tools/train_speed.py compares widths)
 }
 
 // ---- tensor-core path: operand staging + warp-specialised GEMMs ------------------------------------
@@ -1872,16 +1871,17 @@ static bool fused_staging(const vk_vae *net, int B) {
     return true;
 }
 
-// Cluster fold (see fold_cluster_sums): on for 2..4 row tiles (B <= 512) unless VK_CLUSTER_FOLD=0.  Measured step times
-// (tools/train_speed.py, us, cluster fold / grid barrier): B = 256: 180.5 / 199.0, 512: 203.8 / 219.0, and with clusters
-// of 8 at B = 1024: 307.3 / 274.8 -- eight co-scheduled 1-CTA-per-SM blocks per GPC cost more than the barrier saves.
+// Cluster fold (see fold_cluster_sums): on for 2 row tiles (129 <= B <= 256) unless VK_CLUSTER_FOLD=0.  Larger clusters of
+// co-scheduled 1-CTA-per-SM blocks are harder to place on a GPC than the software barrier they replace costs: on an
+// H100 SXM (400 W power limit, tools/train_speed.py, us per step, cluster fold / grid barrier) B = 256: 195 / 208, but
+// B = 512 (clusters of 4): 257 / 248.
 static int cluster_fold_rt(int B) {
     static const int on = [] {
         const char *v = getenv("VK_CLUSTER_FOLD");
         return v ? atoi(v) : 1;
     }();
     const int rt = (B + 127) / 128;
-    return (on && rt >= 2 && rt <= 4) ? rt : 0;
+    return (on && rt == 2) ? rt : 0;
 }
 
 static int launch_prep(const PrepArgs &a, cudaStream_t s) {

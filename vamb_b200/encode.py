@@ -1,4 +1,4 @@
-__doc__ = """Encode a depths matrix and a tnf matrix to latent representation on B200.
+__doc__ = """Encode a depths matrix and a tnf matrix to latent representation on H100.
 
 Drop-in for ``vamb.encode`` (RasmussenLab/vamb, vamb/encode.py): ``make_dataloader``,
 ``set_batchsize`` and ``VAE`` keep the reference's names, arguments, attributes,
@@ -6,7 +6,7 @@ Drop-in for ``vamb.encode`` (RasmussenLab/vamb, vamb/encode.py): ``make_dataload
 
   * the normalised dataset is uploaded to HBM once; minibatches are drawn on the device by
     an epoch-keyed pseudo-random permutation (no DataLoader worker, no per-step H2D);
-  * one optimiser step = 15 hand-written sm_100a kernel launches (vamb_b200/csrc/vk_vae.cu)
+  * one optimiser step = 15 hand-written sm_90a kernel launches (vamb_b200/csrc/vk_vae.cu)
     -- batch gather, fused Linear+LeakyReLU+Dropout+BatchNorm forward, loss, fused
     backward, single-pass D-Adaptation Adam -- replayed from CUDA graphs, with the five
     loss scalars accumulated on the device and read once per epoch;
@@ -57,9 +57,9 @@ def _warn_once(msg: str) -> None:
 
 _MAX_BATCH = 8192  # rows of the activation workspaces (training batches double up to 4096)
 _GRAPH_CHUNKS = (128, 16, 4)  # optimiser steps per captured CUDA graph, largest first
-_WGRAD_FLUSH = 0  # default of vk_vae.wgrad_flush: measured against fp64 the plain chain is already at 8.5e-6 (profiles/r02_grad_error_fp64.txt)
-_USE_TMA = 1  # default of vk_vae.use_tma: validated on B200 (tests/test_vae_gpu.py, test_tc_gpu.py), 1-7 % faster steps
-_TC_MIN_BATCH = 128  # batches >= this run their GEMMs on the tcgen05 tensor-core path (0 = never)
+_WGRAD_FLUSH = 0  # default of vk_vae.wgrad_flush: the plain chain is fp32-grade against fp64 (tools/grad_error_fp64.py)
+_USE_TMA = 1  # default of vk_vae.use_tma (both feeds are checked by tests/test_vae_gpu.py, test_tc_gpu.py)
+_TC_MIN_BATCH = 128  # batches >= this run their GEMMs on the wgmma tensor-core path (0 = never)
 
 
 def set_batchsize(data_loader: _DataLoader, batch_size: int, n_obs: int, encode=False) -> _DataLoader:
@@ -313,7 +313,7 @@ class VAE(_nn.Module):
         if not cuda:
             # The reference's default (cuda=False) selects its CPU path.  This implementation has none -- it IS the
             # GPU path -- so the flag cannot be honoured; say so once instead of silently ignoring it.
-            _warn_once("vamb_b200.encode.VAE always runs on the GPU (sm_100a); cuda=False is not honoured")
+            _warn_once("vamb_b200.encode.VAE always runs on the GPU (sm_90a); cuda=False is not honoured")
 
         # Parameters are drawn by CPU torch in the reference's construction order
         # (vamb/encode.py:210-249) so that the same seed gives the same initial weights.

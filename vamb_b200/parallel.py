@@ -10,7 +10,7 @@ The exchange steps are tiny and latency-bound, so they are kept to the minimum t
 * clustering: independent per shard ("bins are split per sample"); no collective.
 
 The helpers are backend-agnostic so that the host logic is covered by world_size-2 gloo tests on CPU
-(tests/test_parallel_cpu.py); on the GPU box the backend is NCCL over NVLink.
+(tests/test_parallel_cpu.py); on GPUs the backend is NCCL over NVLink.
 """
 from __future__ import annotations
 
